@@ -3,6 +3,7 @@
 3 source views, 18 keypoints).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config {2,3,4,5}] [--scene {ones,hull}] [--impl reference]
+                    [--dump-outputs DIR]
 
 A step = one pass of the hot path over one synthetic frame: re-layout of the (new) source feature
 maps + ray generation + sampling + shading + compositing for every pixel of the novel view.
@@ -17,12 +18,14 @@ The frames are exchanged with ONE NCCL all-gather.
 `value`   : inputs resident in HBM, CUDA-event time on the launch stream, max over ranks.
 `e2e`     : the same metric through the reference-facing API (`KeypointNeRF.render_pifu_nerf`) with
             pinned HOST tensors in and host tensors out (H2D + D2H inside the timed region).
-`roofline`: the dominant kernel (shade_geo_vseq_kernel at 18 keypoints, shade_geo_kernel at 24): algorithmic FLOPs of the samples it shaded / its device time, both
+`roofline`: the dominant kernels (geo_front_kernel + geo_tail_kernel): algorithmic FLOPs of the samples they shaded / their device time, both
             measured live (valid-sample counter of the launch, CUDA events around the kernel on the launch stream inside the
             timed region), against the measured dense bf16 tensor peak in MEASURED_PEAKS.json; `pair` adds the colour kernel
             (executed FLOPs: 419 200 per valid sample + 79 536 per sample with density > 0).
 `cpu_baseline` / `--impl reference`: the CPU oracle port (oracle/, torch-CPU, all host threads) on a bounded sample of the
             same workload (a strided pass of the same frame: 4096 rays, fewer when that would take too long).
+`--dump-outputs DIR`: after the timed steps, the arrays the render call of the last timed step returned (and, with N > 1, the
+            gathered frame) as DIR/<name>.npy in float32.  The inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -82,7 +85,7 @@ def peaks():
         d = json.load(open(p))
         return {"tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops"))), "hbm_gbs": float(d["hbm_gbs"]),
                 "source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"}
-    return {"tflops": 1400.0, "hbm_gbs": 6650.0, "source": "B200_PROFILING.md fallback, sustained (of fallback)"}
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet, dense bf16 (not measured)"}
 
 
 class ClockSampler:
@@ -196,6 +199,17 @@ def run_reference_arm(args, cfg, out_fd):
     return 0
 
 
+def dump_outputs(directory: str, res: dict, frame):
+    """What the timed path returned in its last step, as float32 .npy files (a 512x512 frame's outputs are a few MB)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    arrays = {k: v for k, v in res.items() if hasattr(v, "detach")}
+    if frame is not None:
+        arrays["gathered_frame"] = frame
+    for name, t in sorted(arrays.items()):
+        np.save(os.path.join(directory, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def _private_stdout():
     """The contract is ONE JSON line on stdout: libraries (NCCL prints its version banner there) get stderr instead."""
     sys.stdout.flush()
@@ -223,6 +237,7 @@ def main():
     ap.add_argument("--n-kpt", type=int, default=N_KPT)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-steps", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     if args.impl == "reference":
@@ -258,7 +273,7 @@ def main():
     h = scene_tensors(scene, target, "cpu", pin=True)
     m = net.marcher()
     m.reserve(size * size // (world if lattice else 1), S_c + S_f)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # several times the 50 MB L2
     kw = dict(S_c=S_c, S_f=S_f, fine=fine, engine=args.engine, ert_eps=ert)
     key = "tex_fg_fine" if fine else "tex_fg"
     gev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
@@ -288,6 +303,7 @@ def main():
             out = D.gather_views(res[key], world)
         if k >= 0:
             gev[k][1].record()
+        gstate["res"], gstate["frame"] = res, out
         return out
 
     cfgk = dict(sample_per_ray_c=S_c, sample_per_ray_f=S_f, fine=fine, uniform=True, ert_eps=ert)
@@ -327,6 +343,8 @@ def main():
     gstate["k"] = -1
     barrier()
     t_wall = time.perf_counter() - t_wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, gstate["res"], gstate["frame"] if world > 1 else None)
     clocks = sampler.stop()
     st = m.stats()   # counters of the LAST step's render, event times summed over the timed steps
     m.set_profiling(False)
@@ -370,8 +388,7 @@ def main():
     ach_geo = f_geo * valid * args.steps / (geo_ms * 1e-3) / 1e12 if geo_ms > 0 else None
     ach_pair = (f_geo * valid + f_ibr * coloured) * args.steps / (shade_ms * 1e-3) / 1e12 if shade_ms > 0 else None
     t_geo, t_pair, t_src = ncu_traffic()
-    vseq = n_kpt == 18 and args.engine in (0, 3)   # the library's choice of geometry kernel (include/kpnerf_b200.h, kpn_opts.engine)
-    gk = "shade_geo_vseq_kernel" if vseq else "shade_geo_kernel"
+    gk = "geo_front_kernel + geo_tail_kernel"
     roofline = {"bound": "tensor", "kernel": gk + " (gather + keypoint encoding + geometry MLP + pooling + density tail)",
                 "achieved": ach_geo, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": (ach_geo / pk["tflops"]) if ach_geo else None,
                 "traffic": t_geo, "traffic_unit": "DRAM bytes per launch (one chunk = one 512x512x128 frame), ncu --set full",

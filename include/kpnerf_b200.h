@@ -1,5 +1,5 @@
 /*
- * kpnerf_b200 -- C ABI of the B200-native KeypointNeRF ray-march hot path.
+ * kpnerf_b200 -- C ABI of the CUDA-native (H100, sm_90a) KeypointNeRF ray-march hot path.
  *
  * The reference (facebookresearch/KeypointNeRF) has no FFI: its seam for this path is
  * the Python method surface of class KeypointNeRF (SURVEY.md section 8b).  Each entry
@@ -118,14 +118,14 @@ typedef struct {
   int fine;               /* config["fine"] */
   float ert_eps;          /* early-ray-termination transmittance threshold; 0 = off (reference behaviour) */
   const float* z_fine_override; /* optional (R, S_c+S_f) sorted depths replacing the resampled ones (test hook; same kpn_mem as kpn_out) */
-  int engine;             /* 0 = default: tcgen05, fp16 operands with two-term (hi+lo) weights, fp32 accumulate; the geometry
-                                 kernel is the view-sequential one for n_kpt == 18 and the row-per-view one for n_kpt == 24;
+  int engine;             /* 0 = default: tensor cores (wgmma), fp16 operands, fp32 accumulate; the density tail (stages P0|compress,
+                                 P1) runs with two-term (hi+lo) weights and activations;
                              1 = fp32 CUDA-core engine (parity anchor, ~25x slower; the ONLY engine for shapes the tensor-core
                                  engine does not cover: n_views != 3, n_kpt not in {18,24}, sp_level != 3 -- such shapes
                                  fail with KPN_ERR_UNSUPPORTED unless engine = 1 is requested explicitly);
-                             2 = tcgen05 (row-per-view geometry kernel) with single-term fp16 weights (~2x the rounding error);
-                             3 = as 0 but the view-sequential geometry kernel explicitly (KPN_ERR_UNSUPPORTED if n_kpt != 18);
-                             4 = as 0 but the row-per-view geometry kernel explicitly */
+                             2 = as 0 with single-term fp16 weights in the density tail (more rounding error);
+                             3, 4 = as 0 (they selected between two geometry kernels of an earlier architecture; one kernel
+                                 serves both here) */
 } kpn_opts;
 
 /* Outputs of batch_render_pifu_nerf (reference src/model.py:1065-1096); any pointer may be NULL. */
@@ -214,19 +214,21 @@ int kpn_debug_timing(kpn_ctx* ctx, int enable, unsigned long long* out16);
  * {18, 24}: kmap_out[i] = K index input i is multiplied with, *kbias_out = K index of the bias row, *kpad_out = padded K. */
 int kpn_debug_kmap(int stage, int n_kpt, int n_inputs, int* kmap_out, int* kbias_out, int* kpad_out);
 
-/* Debug, instrumented build (-DKPN_STAGE_TIMING, tools/stage_times.py) only: per-stage cycle stamps of one issuer warp of the
- * geometry kernel; KPN_ERR_UNSUPPORTED in the normal build. */
+/* Debug hook kept for ABI stability: per-stage cycle stamps of an instrumented build; no instrumented build of the
+ * current kernels exists, so it returns KPN_ERR_UNSUPPORTED. */
 int kpn_debug_stage_times(kpn_ctx* ctx, unsigned long long* out, int n_words, int* n_tiles);
 
 /* enable != 0: bracket every shading-kernel launch with CUDA events on its stream (no sync). */
 int kpn_set_profiling(kpn_ctx* ctx, int enable);
 
 /* Unit test hook for the tensor-core primitive (tests/test_gpu_umma.py): D(128,N) fp32 = A(128,K) fp16 * B(N,K)^T fp16
- * on one CTA through tcgen05.mma.  Device pointers.  variant bit0: B core-matrix arrangement, bit1: A from shared memory. */
+ * on one warpgroup through wgmma.mma_async (two 64-row MMAs), operands in the shared-memory layouts the kernels use.
+ * Device pointers.  N in {16, 32, 48, 64, 96, 112, 128, 144, 192}, K % 16 == 0, K <= 256; variant must be 0. */
 int kpn_selftest_umma(int N, int K, const void* A, const void* B, float* D, int variant, void* stream);
-/* Same for the CTA-pair form (cta_group::2): D(256,N) = A(256,K) * B(N,K)^T on a 2-CTA cluster, with the activation tile at
- * tensor-memory column a_col and the accumulator at d_col (the geometry kernel's placements), issued by one thread (mode 0),
- * warp-converged with an elected lane and predicated MMAs (mode 1, what the kernels use) or by the elected lane in a branch (2). */
+/* Same on a 2-CTA cluster: D(256,N) = A(256,K) * B(N,K)^T, each CTA holding half of B's rows and fetching the other half from
+ * its peer's shared memory (distributed shared memory) before its wgmma; N in {32, 64, 96, 128, 192}.  The activation tile is
+ * d_col 32-bit columns wide with A at columns [a_col, a_col + K/2); mode 0 / 1 / 2: the peer's half is read remotely / pushed
+ * by one bulk copy completing on an mbarrier / written by remote stores. */
 int kpn_selftest_umma2(int N, int K, const void* A, const void* B, float* D, int a_col, int d_col, int mode, void* stream);
 
 #ifdef __cplusplus

@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# KPN_LIB selects an alternative build of the same ABI (the instrumented library of tools/stage_times.py)
+# KPN_LIB selects an alternative build of the same ABI (e.g. one built with extra -D flags for an experiment)
 LIB_PATH = os.environ.get("KPN_LIB") or os.path.join(_HERE, "lib", "libkpnerf_b200.so")
 
 KPN_OK = 0

@@ -1,6 +1,6 @@
 // C ABI of the ray-march path (include/kpnerf_b200.h): context, weight packer, scene packer,
 // render / query drivers.  Host logic only; kernels live in kpn_kernels.cu (fp32 SIMT engine)
-// and kpn_tc.cu (tensor-core engine).
+// and kpn_shade_tc.cu (tensor-core engine).
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
@@ -44,7 +44,7 @@ struct DeviceGuard {
 
 struct kpn_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::string err;
   bool have_weights = false, have_scene = false;
   int n_kpt = 0;
@@ -58,8 +58,7 @@ struct kpn_ctx {
   DevWeightsF32* d_wf32 = nullptr;
   DevBuf wbuf;
   DevBuf wblob;                // fp16 weight tiles of the tensor-core engine (core-matrix layout)
-  DevBuf wlo;                  // per-CTA-rank half-blobs [W_hi halves | W_lo halves] of the geometry stages (CTA-pair kernel)
-  DevBuf wlo_vs;               // the same for the view-sequential kernel (different layer-0 input permutation)
+  DevBuf wlo;                  // fp16 W_lo tiles of the density-tail stages 4, 5 (same layout as their W_hi tiles)
   TcConsts tcc;                // fp32 constants of the tensor-core engine (kernel parameter)
   bool tc_weights = false;
   int scene_views = 0;
@@ -73,7 +72,7 @@ struct kpn_ctx {
   DevBuf atlas_fg;
   // per-chunk workspace: rays (dir, near/far), per-ray list ranges of up to two segments, the work list, the compact per-sample
   // records (alpha+sdf, rgb, compositing weight), the fine depths, the colour kernel's latent scratch + work list
-  DevBuf ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib;
+  DevBuf ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
   DevBuf ws_out, ws_in;
   unsigned long long launches = 0;
   bool profiling = false;
@@ -137,12 +136,11 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   c->wbuf.release();
   c->wblob.release();
   c->wlo.release();
-  c->wlo_vs.release();
   for (auto& b : c->stage) b.release();
   for (auto& b : c->atlas) b.release();
   c->atlas_fg.release();
   for (DevBuf* b : {&c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
-                    &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_out, &c->ws_in})
+                    &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in})
     b->release();
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   if (c->h_wd) cudaFreeHost(c->h_wd);
@@ -243,47 +241,31 @@ extern "C" int kpn_set_weights(kpn_ctx* c, const kpn_weights* w) {
   if (tc_supported(3, w->n_kpt, w->sp_level)) {
     const TcPlan plan = make_tc_plan(w->n_kpt);
     std::vector<__half> blob(plan.total_bytes / 2, __float2half_rn(0.0f));
-    const size_t geo_bytes = tc_weight_lo_bytes(w->n_kpt);          // bytes of the full W_hi tiles of stages 0..5
-    std::vector<__half> pair(tc_pair_blob_bytes(w->n_kpt) / 2, __float2half_rn(0.0f));   // [rank][hi halves | lo halves]
-    const bool vseq = vs_run_cols(w->n_kpt) > 0;
-    std::vector<__half> pair_vs(vseq ? pair.size() : 0, __float2half_rn(0.0f));           // view-sequential kernel: same tiles, other K permutation
+    std::vector<__half> lo(tc_weight_lo_bytes(w->n_kpt) / 2, __float2half_rn(0.0f));   // W_lo = fp16(W - W_hi) of stages 4, 5
     // stage -> (layer, first row in the tile); stage 4 stacks the density layer 0 and the colour compress layer
     const int stage_layer[TC_NSTAGE] = {L_GEO0, L_GEO1, L_GEO2, L_GEO3, L_DEN0, L_DEN1, L_BASE0, L_BASE1, L_VIS1A, L_VIS1B, L_VIS2A, L_OUT0, L_RE1};
-    auto put_pair = [&](std::vector<__half>& dst, int stage, int n, int kk, float wv) {
-      // geometry stages: row n of the tile goes to CTA rank n / (Np/2), as row n % (Np/2) of its half tile
-      const int Np = plan.st[stage].Np, Nh = Np / 2, rk = n / Nh;
-      const size_t half_at = ((size_t)rk * geo_bytes + plan.st[stage].off / 2 + tc::core_offset_bytes(n % Nh, kk, Nh)) / 2;
-      const __half hi = __float2half_rn(wv);
-      dst[half_at] = hi;
-      dst[half_at + geo_bytes / 4] = __float2half_rn(wv - __half2float(hi));   // lo halves follow the hi halves
-    };
     auto put_one = [&](int stage, int n, int kk, float wv) {
       const int Np = plan.st[stage].Np;
       const size_t at = (plan.st[stage].off + tc::core_offset_bytes(n, kk, Np)) / 2;
-      blob[at] = __float2half_rn(wv);
-      if (stage < 6) put_pair(pair, stage, n, kk, wv);
+      const __half hi = __float2half_rn(wv);
+      blob[at] = hi;
+      if (stage == 4 || stage == 5) lo[at - plan.st[4].off / 2] = __float2half_rn(wv - __half2float(hi));
     };
     auto put = [&](int stage, int layer, int row0) {
       const kpn_layer& L = w->layer[layer];
       for (int o = 0; o < L.n_out; ++o) {
         for (int i = 0; i < L.n_in; ++i) {
           put_one(stage, row0 + o, stage < 6 ? tc_kmap(stage, w->n_kpt, i) : i, We[layer][(size_t)o * L.n_in + i]);
-          if (vseq && stage < 6) put_pair(pair_vs, stage, row0 + o, tc_kmap_vseq(stage, w->n_kpt, i), We[layer][(size_t)o * L.n_in + i]);
         }
         if (stage < 6 || stage == 12) put_one(stage, row0 + o, tc_kbias(stage, w->n_kpt), L.bias[o]);   // bias row (activation column == 1)
-        if (vseq && stage < 6) put_pair(pair_vs, stage, row0 + o, tc_kbias_vseq(stage, w->n_kpt), L.bias[o]);
       }
     };
     for (int sidx = 0; sidx < TC_NSTAGE; ++sidx) put(sidx, stage_layer[sidx], 0);
     put(4, L_CMP, 64);
     KPN_CUDA(c, c->wblob.reserve(plan.total_bytes));
     KPN_CUDA(c, cudaMemcpy(c->wblob.p, blob.data(), plan.total_bytes, cudaMemcpyHostToDevice));
-    KPN_CUDA(c, c->wlo.reserve(pair.size() * 2));
-    KPN_CUDA(c, cudaMemcpy(c->wlo.p, pair.data(), pair.size() * 2, cudaMemcpyHostToDevice));
-    if (vseq) {
-      KPN_CUDA(c, c->wlo_vs.reserve(pair_vs.size() * 2));
-      KPN_CUDA(c, cudaMemcpy(c->wlo_vs.p, pair_vs.data(), pair_vs.size() * 2, cudaMemcpyHostToDevice));
-    }
+    KPN_CUDA(c, c->wlo.reserve(lo.size() * 2));
+    KPN_CUDA(c, cudaMemcpy(c->wlo.p, lo.data(), lo.size() * 2, cudaMemcpyHostToDevice));
     TcConsts& T = c->tcc;
     memset(&T, 0, sizeof(T));
     auto bias = [&](int layer, float* dst) { for (int o = 0; o < w->layer[layer].n_out; ++o) dst[o] = w->layer[layer].bias[o]; };
@@ -416,15 +398,12 @@ static int shade_batch(kpn_ctx* c, const SampleSrc& src, const int* list, const 
   if (use_tc) {
     KPN_CUDA(c, c->ws_lat.reserve((size_t)n * 48));
     KPN_CUDA(c, c->ws_list2.reserve((size_t)n * 8));
-    // geometry kernel: the view-sequential one where it is built (18 keypoints), else the row-per-view one; 3 / 4 force either
-    const bool vs_built = vs_run_cols(c->n_kpt) > 0;
-    if (engine == 3 && !vs_built)
-      KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "engine 3 (view-sequential geometry kernel) is built for n_kpt == 18; this scene has %d", c->n_kpt);
-    const bool vs = vs_built && (engine == 0 || engine == 3);
-    KPN_CUDA(c, launch_shade_tc(c->d_scene, c->tcc, c->wblob.as<uint8_t>(), vs ? c->wlo_vs.as<uint8_t>() : c->wlo.as<uint8_t>(),
-                                engine == 2 ? 0 : 1, vs ? -c->n_kpt : c->n_kpt, src, list, counter, n, query_mode, so, c->ws_lat.p,
-                                c->ws_list2.p, counter2, c->num_sms, em, st));
-    c->launches += 2;
+    KPN_CUDA(c, c->ws_pool.reserve(tc_pool_bytes(n)));
+    int launches = 0;
+    KPN_CUDA(c, launch_shade_tc(c->d_scene, c->tcc, c->wblob.as<uint8_t>(), c->wlo.as<uint8_t>(), engine == 2 ? 0 : 1, c->n_kpt, src,
+                                list, counter, n, query_mode, so, c->ws_lat.p, c->ws_pool.p, c->ws_list2.p, counter2, c->num_sms, em,
+                                &launches, st));
+    c->launches += launches;
   }
   else {
     KPN_CUDA(c, launch_shade_simt(c->d_scene, c->d_wf32, src, list, counter, n, query_mode, so, c->num_sms, st));

@@ -100,7 +100,7 @@ cudaError_t launch_decode_views(const uint8_t* images, const uint8_t* masks, con
                                 float* out_img, uint8_t* out_mask, cudaStream_t st) {
   const long long n = (long long)V * (H0 / factor) * (W0 / factor);
   long long g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (g < 1) g = 1;
   decode_views_kernel<<<(int)g, 256, 0, st>>>(images, masks, reinterpret_cast<const DecodeView*>(cams), V, H0, W0, factor, out_img, out_mask);
   return cudaGetLastError();

@@ -920,7 +920,7 @@ static inline int grid_for(long long n, int block, int cap) {
 
 cudaError_t launch_pack_nhwc_f32(const float* in, float* out, int V, int C, int H, int W, int Cp, cudaStream_t st) {
   long long n = (long long)V * H * W * Cp;
-  pack_nhwc_f32_kernel<<<grid_for(n, 256, 148 * 16), 256, 0, st>>>(in, out, V, C, H, W, Cp);
+  pack_nhwc_f32_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(in, out, V, C, H, W, Cp);
   return cudaGetLastError();
 }
 cudaError_t launch_prep_scene(const RawScene* raw, DevScene* sc, cudaStream_t st) {
@@ -945,7 +945,7 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, front_kernel, FRONT_THREADS, 0) != cudaSuccess || bps < 1) bps = 4;
     per_sm.store(bps, std::memory_order_release);
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int nwords = (S + 31) / 32;
@@ -956,7 +956,7 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr
 }
 cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out5,
                            uint8_t* valid_out, cudaStream_t st) {
-  compact_kernel<<<grid_for(n, 256, 148 * 16), 256, 0, st>>>(sc, src, n, list, counter, out5, valid_out);
+  compact_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(sc, src, n, list, counter, out5, valid_out);
   return cudaGetLastError();
 }
 cudaError_t launch_shade_simt(const DevScene* sc, const DevWeightsF32* W, const SampleSrc& src, const int* list,
@@ -979,7 +979,7 @@ cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb
                              long long plane, float* color, float* depth, float* alpha, float* sdf, float* ray_alpha, float* cw,
                              cudaStream_t st) {
   const RaySeg s0{start0, cnt0}, s1{start1, cnt1};
-  composite_kernel<<<grid_for((long long)nr * 32, 128, 148 * 64), 128, 0, st>>>(list, ao, rgb, s0, s1, start1 ? 2 : 1, zbuf, ray_nf, r0, nr,
+  composite_kernel<<<grid_for((long long)nr * 32, 128, 132 * 64), 128, 0, st>>>(list, ao, rgb, s0, s1, start1 ? 2 : 1, zbuf, ray_nf, r0, nr,
                                                                                S, plane, color, depth, alpha, sdf, ray_alpha, cw);
   return cudaGetLastError();
 }
@@ -995,7 +995,7 @@ cudaError_t launch_resample(const int* list, const float* cw, const int* start0,
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
-  resample_kernel<<<grid_for(nr, RES_WARPS, 148 * 16), RES_WARPS * 32, smem, st>>>(list, cw, s0, s1, start1 ? 2 : 1, ray_nf, nr, Sc, Sf, zout,
+  resample_kernel<<<grid_for(nr, RES_WARPS, 132 * 16), RES_WARPS * 32, smem, st>>>(list, cw, s0, s1, start1 ? 2 : 1, ray_nf, nr, Sc, Sf, zout,
                                                                                contrib_out);
   return cudaGetLastError();
 }

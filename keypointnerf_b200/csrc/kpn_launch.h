@@ -23,18 +23,19 @@ cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb
                              cudaStream_t st);
 cudaError_t launch_resample(const int* list, const float* cw, const int* start0, const int* cnt0, const int* start1, const int* cnt1,
                             const float* ray_nf, int nr, int Sc, int Sf, float* zout, float* contrib_out, cudaStream_t st);
-// Tensor-core engine: geometry+density kernel (CTA pairs), then the colour kernel on the samples with density > 0.
-// wblob: full fp16 W_hi tiles (colour stages are read from it); wpair: per-CTA-rank half-blobs [W_hi halves | W_lo halves] of the
-// geometry stages; lat_scratch: n_max x 48 bytes, list2: n_max x int2, count2: device int (zeroed by the caller).
-cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wpair, int two_term, int n_kpt,
+// Tensor-core engine: geometry front (L0-L3 + pooling) and density tail kernels, then the colour kernel on the samples with
+// density > 0.  wblob: full fp16 W_hi tiles of every stage; wlo: W_lo tiles of stages 4, 5 (tc_weight_lo_bytes);
+// lat_scratch: n_max x 48 bytes, pool_scratch: tc_pool_bytes(n_max), list2: n_max x int2, count2: device int (zeroed by the
+// caller).  *launches is incremented by the number of kernels enqueued.
+cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term, int n_kpt,
                             const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                            const ShadeOut& so, void* lat_scratch, void* list2, int* count2, int num_sms, cudaEvent_t after_geo,
-                            cudaStream_t st);
-size_t tc_pair_blob_bytes(int n_kpt);
+                            const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
+                            cudaEvent_t after_geo, int* launches, cudaStream_t st);
+size_t tc_pool_bytes(long long n_max);
 cudaError_t tc_watchdog_read(unsigned int out[8], bool reset);
 cudaError_t tc_watchdog_read_async(unsigned int* pinned_out8, cudaStream_t st);   // stream-ordered copy into pinned host memory
 cudaError_t tc_watchdog_clear_async(cudaStream_t st);
-cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles);   // instrumented build only
+cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles);   // not supported: cudaErrorNotSupported
 size_t tc_weight_blob_bytes(int n_kpt);
 size_t tc_weight_lo_bytes(int n_kpt);
 bool tc_supported(int n_views, int n_kpt, int sp_level);

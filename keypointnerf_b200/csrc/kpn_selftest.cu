@@ -1,190 +1,182 @@
-// Self-test of the tensor-core primitive used by the ray-march engine: one 128 x N x K fp16 GEMM tile
-// with fp32 accumulation, D[128][N] = A[128][K] * B[N][K]^T, through tcgen05.mma with the A operand in
-// tensor memory (written with tcgen05.st exactly as the activation epilogues do) and the B operand in
-// shared memory in the interleaved core-matrix layout the weight packer emits.  Exercised by
-// tests/test_gpu_umma.py against torch.matmul; it pins the descriptor encodings independently of the
-// network kernels.
+// Self-tests of the tensor-core primitive used by the ray-march engine.  One 128 x N x K fp16 GEMM tile with fp32
+// accumulation, D[128][N] = A[128][K] * B[N][K]^T, through wgmma.mma_async with the A operand in the activation-tile layout
+// the kernels' epilogues write (tc::a_word_off) and the B operand in the interleaved core-matrix layout the weight packer
+// emits.  One warpgroup issues the two 64-row halves.  Exercised by tests/test_gpu_umma.py against torch.matmul; it pins
+// the descriptor encodings and the accumulator fragment layout independently of the network kernels.
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include "kpn_tc.cuh"
 
 namespace kpn {
 
-// variant bit0: B arrangement 0 = [k/8][n/8] (LBO=(N/8)*128, SBO=128), 1 = [n/8][k/8] (LBO=128, SBO=(K/8)*128)
-// variant bit1: A operand 0 = tensor memory, 1 = shared memory (same arrangement rule as B, 128 rows)
+template <int N>
 __global__ void __launch_bounds__(128, 1)
-umma_selftest_kernel(int N, int K, const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D, int variant) {
+wgmma_selftest_kernel(int K, const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
-  const int t = threadIdx.x, warp = t >> 5;
+  const int t = threadIdx.x, w = t >> 5, l = t & 31;
   uint8_t* sB = smem;
   uint8_t* sA = smem + (size_t)N * K * 2;
-  const bool b_alt = variant & 1, a_smem = variant & 2;
-
-  if (warp == 0) tc::tmem_alloc(&tmem_base_s, 512);
-  if (t == 0) { tc::mbar_init(&bar, 1); tc::fence_mbar_init(); }
   for (int idx = t; idx < N * K; idx += 128) {
-    int n = idx / K, k = idx % K;
-    uint32_t off = b_alt ? (uint32_t)(((n >> 3) * (K >> 3) + (k >> 3)) * 128 + (n & 7) * 16 + (k & 7) * 2)
-                         : tc::core_offset_bytes(n, k, N);
-    *reinterpret_cast<__half*>(sB + off) = B[idx];
+    const int n = idx / K, k = idx % K;
+    *reinterpret_cast<__half*>(sB + tc::core_offset_bytes(n, k, N)) = B[idx];
   }
-  if (a_smem) {
-    for (int idx = t; idx < 128 * K; idx += 128) {
-      int n = idx / K, k = idx % K;
-      uint32_t off = b_alt ? (uint32_t)(((n >> 3) * (K >> 3) + (k >> 3)) * 128 + (n & 7) * 16 + (k & 7) * 2)
-                           : tc::core_offset_bytes(n, k, 128);
-      *reinterpret_cast<__half*>(sA + off) = A[idx];
-    }
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t lane_base = tbase + ((uint32_t)(warp * 32) << 16);
-  const uint32_t a_col = 0, d_col = 256;
-  if (!a_smem) {
-    const __half* arow = A + (size_t)t * K;
-    for (int kc = 0; kc < K / 16; ++kc) {
-      uint32_t r[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) r[i] = tc::pack_h2(__half2float(arow[kc * 16 + 2 * i]), __half2float(arow[kc * 16 + 2 * i + 1]));
-      tc::tmem_st8(lane_base + a_col + kc * 8, r);
-    }
-    tc::wait_st();
+  for (int idx = t; idx < 128 * K; idx += 128) {
+    const int r = idx / K, k = idx % K;
+    *reinterpret_cast<__half*>(sA + tc::a_word_off<128>(r, k >> 1) + (k & 1) * 2) = A[idx];
   }
   tc::fence_proxy_async_smem();
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  if (t == 0) {
-    const uint32_t idesc = tc::make_idesc_f16(128, N);
-    const uint32_t lbo_b = b_alt ? 128u : (uint32_t)(N / 8) * 128u, sbo_b = b_alt ? (uint32_t)(K / 8) * 128u : 128u;
-    const uint32_t lbo_a = b_alt ? 128u : 16u * 128u, sbo_a = b_alt ? (uint32_t)(K / 8) * 128u : 128u;
-    for (int j = 0; j < K / 16; ++j) {
-      uint64_t bd = tc::make_smem_desc(tc::smem_u32(sB) + j * 2 * lbo_b, lbo_b, sbo_b);
-      if (a_smem) {
-        uint64_t ad = tc::make_smem_desc(tc::smem_u32(sA) + j * 2 * lbo_a, lbo_a, sbo_a);
-        tc::mma_ss(tbase + d_col, ad, bd, idesc, j > 0);
-      } else {
-        tc::mma_ts(tbase + d_col, tbase + a_col + j * 8, bd, idesc, j > 0);
-      }
-    }
-    tc::mma_commit(&bar);
-  }
-  tc::mbar_wait(&bar, 0);
-  tc::fence_after_sync();
-  for (int c = 0; c < N; c += 8) {
-    uint32_t r[8];
-    tc::tmem_ld8(lane_base + d_col + c, r);
-    tc::wait_ld();
+  const uint32_t a_lbo = 16u * 128u, b_lbo = (uint32_t)(N / 8) * 128u;
+  for (int half = 0; half < 2; ++half) {
+    float d[N / 2];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) D[(size_t)t * N + c + i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.0f;
+    tc::wg_fence();
+    for (int j = 0; j < K / 16; ++j)
+      tc::Wgmma<N>::mma(d, tc::make_smem_desc(tc::smem_u32(sA) + half * 1024u + 2u * a_lbo * j, a_lbo, 128u),
+                        tc::make_smem_desc(tc::smem_u32(sB) + 2u * b_lbo * j, b_lbo, 128u), j > 0 ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait0();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const int r = 64 * half + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      D[(size_t)r * N + c] = d[i];
+    }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, 512);
 }
 
-// 2-CTA variant: D[256][N] = A[256][K] * B[N][K]^T.  CTA r holds rows 128r..128r+127 of A (TMEM) and rows
-// r*N/2 .. (r+1)*N/2-1 of B (shared memory, [k/8][n/8] core-matrix order with N/2 rows).
+template <int N>
+static int run_selftest(int K, const void* A, const void* B, float* D, cudaStream_t st) {
+  const size_t smem = (size_t)N * K * 2 + (size_t)128 * K * 2;
+  if (cudaFuncSetAttribute(wgmma_selftest_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -2;
+  wgmma_selftest_kernel<N><<<1, 128, smem, st>>>(K, (const __half*)A, (const __half*)B, D);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+
+// CTA-pair form on a 2-CTA cluster: D[256][N] = A[256][K] * B[N][K]^T.  CTA r holds rows 128r .. 128r+127 of A and keeps rows
+// r*N/2 .. (r+1)*N/2-1 of B; the other half of B comes from the peer CTA's shared memory (distributed shared memory), then each
+// CTA multiplies its 128 rows by all of B with wgmma.  B is stored as [n/8][k/8] core matrices (LBO = 128 bytes along K,
+// SBO = (K/8)*128 bytes), so each CTA's half is one contiguous block at the same offset in both CTAs.  The A tile is a_width
+// 32-bit columns wide and A occupies columns [a_col, a_col + K/2) of it.  mode: how the peer's half arrives --
+// 0: this CTA reads it through distributed shared memory, 1: the peer pushes it with one bulk copy that completes on this
+// CTA's mbarrier, 2: the peer writes it with remote stores.
+template <int N>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128, 1)
-umma2_selftest_kernel(int N, int K, const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D, int a_col,
-                      int d_col, int mode) {
+wgmma_pair_selftest_kernel(int K, const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D, int a_col,
+                           int mode) {
+  namespace cg = cooperative_groups;
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t bar_a, bar_acc;
-  __shared__ uint32_t tmem_base_s;
-  const int t = threadIdx.x, warp = t >> 5;
-  const uint32_t rank = tc::cluster_ctarank();
-  const int Nh = N / 2;
-  if (warp == 0) tc::tmem_alloc2(&tmem_base_s, 512);
-  if (t == 0) { tc::mbar_init(&bar_a, 256); tc::mbar_init(&bar_acc, 1); tc::fence_mbar_init(); }
-  for (int idx = t; idx < Nh * K; idx += 128) {
-    int n = idx / K, k = idx % K;
-    *reinterpret_cast<__half*>(smem + tc::core_offset_bytes(n, k, Nh)) = B[(size_t)(rank * Nh + n) * K + k];
+  __shared__ uint64_t bar;
+  cg::cluster_group cl = cg::this_cluster();
+  const uint32_t rank = cl.block_rank(), peer = rank ^ 1u;
+  const int t = threadIdx.x, w = t >> 5, l = t & 31;
+  constexpr int NH = N / 2;
+  const uint32_t half_bytes = (uint32_t)NH * K * 2;
+  uint8_t* sB = smem;
+  uint8_t* sA = smem + 2 * half_bytes;
+  uint8_t* mine = sB + rank * half_bytes;
+  if (t == 0) { tc::mbar_init(&bar, 1); tc::fence_mbar_init(); }
+  for (int idx = t; idx < NH * K; idx += 128) {
+    const int n = idx / K, k = idx % K;
+    *reinterpret_cast<__half*>(mine + ((n >> 3) * (K >> 3) + (k >> 3)) * 128 + (n & 7) * 16 + (k & 7) * 2) =
+        B[(size_t)(rank * NH + n) * K + k];
   }
+  for (int idx = t; idx < 128 * K; idx += 128) {
+    const int r = idx / K, k = idx % K;
+    *reinterpret_cast<__half*>(sA + tc::a_word_off<128>(r, a_col + (k >> 1)) + (k & 1) * 2) = A[(size_t)(rank * 128 + r) * K + k];
+  }
+  __syncthreads();
+  if (mode == 1 && t == 0) tc::mbar_expect_tx(&bar, half_bytes);   // the peer's bulk copy completes this phase
   tc::fence_proxy_async_smem();
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t lane_base = tbase + ((uint32_t)(warp * 32) << 16);
-  const __half* arow = A + (size_t)(rank * 128 + t) * K;
-  for (int kc = 0; kc < K / 16; ++kc) {
-    uint32_t r[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) r[i] = tc::pack_h2(__half2float(arow[kc * 16 + 2 * i]), __half2float(arow[kc * 16 + 2 * i + 1]));
-    tc::tmem_st8(lane_base + a_col + kc * 8, r);
-  }
-  tc::wait_st();
-  tc::fence_before_sync();
-  tc::mbar_arrive_cluster(&bar_a, 0);   // every row thread of both CTAs arrives on the LEADER's barrier
-  const uint32_t idesc = tc::make_idesc_f16(256, N);
-  const uint32_t lbo = (uint32_t)(Nh / 8) * 128u;
-  if (mode == 0) {          // one thread issues
-    if (rank == 0 && t == 0) {
-      tc::mbar_wait(&bar_a, 0);
-      tc::fence_after_sync();
-      for (int j = 0; j < K / 16; ++j) {
-        uint64_t bd = tc::make_smem_desc(tc::smem_u32(smem) + j * 2 * lbo, lbo, 128u);
-        tc::mma_ts2(tbase + d_col, tbase + a_col + j * 8, bd, idesc, j > 0);
-      }
-      tc::mma_commit2(&bar_acc);
+  cl.sync();   // both CTAs: own halves written, barriers initialised
+  if (mode == 0) {
+    const uint8_t* theirs = cl.map_shared_rank(sB + peer * half_bytes, peer);
+    uint8_t* dst = sB + peer * half_bytes;
+    for (uint32_t i = 16u * t; i < half_bytes; i += 16u * 128u)
+      *reinterpret_cast<uint4*>(dst + i) = *reinterpret_cast<const uint4*>(theirs + i);
+    tc::fence_proxy_async_smem();
+    __syncthreads();
+  } else if (mode == 1) {
+    if (t == 0) {
+      uint32_t dst, mb;
+      asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(dst) : "r"(tc::smem_u32(mine)), "r"(peer));
+      asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(mb) : "r"(tc::smem_u32(&bar)), "r"(peer));
+      asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                   ::"r"(dst), "r"(tc::smem_u32(mine)), "r"(half_bytes), "r"(mb) : "memory");
     }
-  } else if (rank == 0 && warp == 0) {   // warp-converged issue: every lane runs the code, the elected lane's MMAs take effect
-    const uint32_t el = tc::elect_one();
-    tc::mbar_wait(&bar_a, 0);
-    tc::fence_after_sync();
-    const uint32_t b0 = ((tc::smem_u32(smem) >> 4) & 0x3FFFu) + ((lbo >> 4) << 16);
-    const uint32_t dhi = (128u >> 4) | (1u << 14);
-    if (mode == 1) {
-      for (int j = 0; j < K / 16; ++j)
-        tc::mma_ts2_el(tbase + d_col, tbase + a_col + j * 8, b0 + (uint32_t)j * ((2u * lbo) >> 4), dhi, idesc, j > 0, el);
-      tc::mma_commit2_el(&bar_acc, el);
-    } else if (el) {                      // mode 2: the elected lane alone takes the branch
-      for (int j = 0; j < K / 16; ++j)
-        tc::mma_ts2_el(tbase + d_col, tbase + a_col + j * 8, b0 + (uint32_t)j * ((2u * lbo) >> 4), dhi, idesc, j > 0, 1u);
-      tc::mma_commit2_el(&bar_acc, 1u);
-    }
-    __syncwarp();
+    tc::mbar_wait(&bar, 0, 0x60u);
+  } else {
+    uint8_t* theirs = cl.map_shared_rank(mine, peer);
+    for (uint32_t i = 16u * t; i < half_bytes; i += 16u * 128u)
+      *reinterpret_cast<uint4*>(theirs + i) = *reinterpret_cast<const uint4*>(mine + i);
+    cl.sync();   // release the remote stores / acquire the peer's
+    tc::fence_proxy_async_smem();
+    __syncthreads();
   }
-  tc::mbar_wait(&bar_acc, 0);
-  tc::fence_after_sync();
-  for (int c = 0; c < N; c += 8) {
-    uint32_t r[8];
-    tc::tmem_ld8(lane_base + d_col + c, r);
-    tc::wait_ld();
+  const uint32_t a0 = tc::smem_u32(sA) + tc::a_word_off<128>(0, a_col), b0 = tc::smem_u32(sB), b_sbo = (uint32_t)(K / 8) * 128u;
+  for (int half = 0; half < 2; ++half) {
+    float d[N / 2];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) D[(size_t)(rank * 128 + t) * N + c + i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.0f;
+    tc::wg_fence();
+    for (int j = 0; j < K / 16; ++j)
+      tc::Wgmma<N>::mma(d, tc::make_smem_desc(a0 + half * 1024u + 4096u * j, 2048u, 128u), tc::make_smem_desc(b0 + 256u * j, 128u, b_sbo),
+                        j > 0 ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait0();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const int r = 128 * (int)rank + 64 * half + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      D[(size_t)r * N + c] = d[i];
+    }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();
-  if (warp == 0) tc::tmem_dealloc2(tbase, 512);
+  cl.sync();   // neither CTA leaves while its peer may still read or write its shared memory
+}
+
+template <int N>
+static int run_pair_selftest(int K, const void* A, const void* B, float* D, int a_col, int a_width, int mode, cudaStream_t st) {
+  const size_t smem = (size_t)N * K * 2 + (size_t)128 * a_width * 4;
+  if (cudaFuncSetAttribute(wgmma_pair_selftest_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return -2;
+  wgmma_pair_selftest_kernel<N><<<2, 128, smem, st>>>(K, (const __half*)A, (const __half*)B, D, a_col, mode);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 }  // namespace kpn
 
-// 2-CTA self-test: A (256,K) fp16, B (N,K) fp16, D (256,N) fp32: device pointers.  N % 32 == 0.  a_col / d_col: tensor-memory
-// columns of the activation tile and the accumulator; mode 0: one issuing thread, 1: warp-converged issue with an elected lane
-// (predicated MMAs), 2: elected lane takes a branch.
+// A (128,K) fp16, B (N,K) fp16, D (128,N) fp32: device pointers.  N in {16, 32, 48, 64, 96, 112, 128, 144, 192} (the widths
+// with a wgmma instantiation), K % 16 == 0, K <= 256.  variant 0 is the only operand arrangement (the one the kernels use).
+extern "C" int kpn_selftest_umma(int N, int K, const void* A, const void* B, float* D, int variant, void* stream) {
+  if (K % 16 || K < 16 || K > 256 || variant != 0) return -1;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (N) {
+    case 16: return kpn::run_selftest<16>(K, A, B, D, st);
+    case 32: return kpn::run_selftest<32>(K, A, B, D, st);
+    case 48: return kpn::run_selftest<48>(K, A, B, D, st);
+    case 64: return kpn::run_selftest<64>(K, A, B, D, st);
+    case 96: return kpn::run_selftest<96>(K, A, B, D, st);
+    case 112: return kpn::run_selftest<112>(K, A, B, D, st);
+    case 128: return kpn::run_selftest<128>(K, A, B, D, st);
+    case 144: return kpn::run_selftest<144>(K, A, B, D, st);
+    case 192: return kpn::run_selftest<192>(K, A, B, D, st);
+    default: return -1;
+  }
+}
+
+// 2-CTA self-test: A (256,K) fp16, B (N,K) fp16, D (256,N) fp32: device pointers.  N in {32, 64, 96, 128, 192}, K % 16 == 0,
+// K <= 256.  The activation tile is d_col 32-bit columns wide with A at columns [a_col, a_col + K/2) (a_col % 8 == 0); mode 0 / 1 / 2:
+// the peer's half of B is read through distributed shared memory / pushed by a bulk copy / written by remote stores.
 extern "C" int kpn_selftest_umma2(int N, int K, const void* A, const void* B, float* D, int a_col, int d_col, int mode, void* stream) {
   if (N % 32 || N < 32 || N > 256 || K % 16 || K < 16 || K > 256) return -1;
   if (a_col < 0 || a_col % 8 || d_col % 8 || a_col + K / 2 > d_col || d_col + N > 512 || mode < 0 || mode > 2) return -1;
-  size_t smem = (size_t)(N / 2) * K * 2;
-  cudaError_t e = cudaFuncSetAttribute(kpn::umma2_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return -2;
-  kpn::umma2_selftest_kernel<<<2, 128, smem, (cudaStream_t)stream>>>(N, K, (const __half*)A, (const __half*)B, D, a_col, d_col, mode);
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
-}
-
-// A (128,K) fp16, B (N,K) fp16, D (128,N) fp32: device pointers.  N % 16 == 0, 16 <= N <= 256, K % 16 == 0.
-extern "C" int kpn_selftest_umma(int N, int K, const void* A, const void* B, float* D, int variant, void* stream) {
-  if (N % 16 || N < 16 || N > 256 || K % 16 || K < 16 || K > 256) return -1;
-  size_t smem = (size_t)N * K * 2 + (size_t)128 * K * 2;
-  cudaError_t e = cudaFuncSetAttribute(kpn::umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return -2;
-  kpn::umma_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(N, K, (const __half*)A, (const __half*)B, D, variant);
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (N) {
+    case 32: return kpn::run_pair_selftest<32>(K, A, B, D, a_col, d_col, mode, st);
+    case 64: return kpn::run_pair_selftest<64>(K, A, B, D, a_col, d_col, mode, st);
+    case 96: return kpn::run_pair_selftest<96>(K, A, B, D, a_col, d_col, mode, st);
+    case 128: return kpn::run_pair_selftest<128>(K, A, B, D, a_col, d_col, mode, st);
+    case 192: return kpn::run_pair_selftest<192>(K, A, B, D, a_col, d_col, mode, st);
+    default: return -1;
+  }
 }

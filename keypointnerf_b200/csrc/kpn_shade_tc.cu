@@ -1,28 +1,25 @@
-// Ray-march shading, engine 0: tcgen05 tensor-core MLPs with activations resident in tensor memory.
+// Ray-march shading, engine 0: Hopper tensor-core MLPs (wgmma, fp16 operands in shared memory, fp32 accumulators in
+// registers, weights resident in shared memory through one bulk-TMA load per CTA).
 //
-// Two persistent kernels per batch of valid samples:
-//   shade_geo_kernel   : gather + keypoint encoding + geometry MLP (L0-L3) + view pooling + density tail (P0|compress, P1,
-//                        64->2 head).  Writes alpha/sdf per sample, the 24-wide compressed latent (fp16) to a scratch buffer,
-//                        and appends the samples that need a colour (density > 0; every valid sample in query mode) to a
-//                        second work list.  A sample with alpha == 0 has compositing weight exactly 0 (src/model.py:1167),
-//                        so skipping its colour is exact.  CTA pairs (cta_group::2), 16 row warps per CTA (2 tile slots x 4
-//                        TMEM lane quarters x 2 column halves), no control warp; see the block comment above geo_dcol.
-//   shade_color_kernel : IBR colour head (RE1, BASE0, BASE1, VIS1A, VIS1B, VIS2A, OUT0 on tensor cores; first ray-encoder
-//                        layer, 32->1, 16->8->1 in fp32 on CUDA cores) for the second list.  One CTA per SM, 4 tile slots x 4
-//                        row warps (row warp 0 of a slot issues its MMAs).
-// Common structure: a row = one (sample, source view) pair, the 3 views of a sample in 3 adjacent lanes (10 samples per
-// warp, 40 per tile) so every cross-view reduction of the reference (view pooling, src/utils.py:722-748; blending weights,
-// mean/var, softmax, src/model.py:1286-1301) is a 3-lane shuffle.  A row thread owns TMEM lane = its row: it writes its layer
-// input as packed fp16 straight into tensor memory (tcgen05.st), the slot's issuer multiplies it with fp16 weights resident
-// in shared memory (bulk-TMA loaded once per CTA) into an fp32 accumulator in another column region, tcgen05.commit ->
-// mbarrier -> the row thread reads its accumulator columns (tcgen05.ld), applies the activation and writes the next layer's
-// fp16 input.  Activations never touch shared or global memory.  Slots ping-pong so the tensor pipe works on one tile while
-// the CUDA cores run another's epilogue.
+// Three persistent kernels per batch of valid samples:
+//   geo_front_kernel  : gather + keypoint encoding + geometry MLP (L0-L3) + view pooling.  A row is one (sample, source view)
+//                       pair; the 3 views of a sample sit in 3 adjacent lanes (10 samples per warp), so the pooling (reference
+//                       src/utils.py:722-748) is a 3-lane shuffle.  Writes the pooled [mean | var] (fp32) of every sample to a
+//                       scratch buffer.
+//   geo_tail_kernel   : density tail per sample (P0|compress, P1 with two-term fp16 weights W_hi + W_lo and two-term
+//                       activations, 64->2 head in fp32).  Writes alpha/sdf and, where a colour is needed, the 24-wide
+//                       compressed latent (fp16).  The tail is a kernel of its own because the geometry stages' W_hi tiles and
+//                       the tail's W_hi + W_lo tiles do not fit in one SM's 227 KB of shared memory together with the tiles.
+//   shade_color_kernel: IBR colour head (RE1, BASE0, BASE1, VIS1A, VIS1B, VIS2A, OUT0 on tensor cores; first ray-encoder layer,
+//                       32->1, 16->8->1 in fp32 on CUDA cores) for the samples with density > 0 (colour_list_kernel's list).
+// Common structure: a warpgroup (4 warps) owns a tile of rows.  Row threads build a layer input as packed fp16 pairs in an
+// activation tile in shared memory (tc::a_word_off layout), the warpgroup multiplies it with the resident weights
+// (wgmma.mma_async, M = 64 per instruction), and the epilogue either runs on the accumulator fragments directly (elementwise
+// activations, written straight into the next layer's activation tile) or stores them to shared memory for the row threads
+// (cross-view reductions).  Biases ride in the MMAs as one extra K row multiplied by a constant 1 in the activation tile.
 // Stage table:
 //   geo    0 L0 190->128 | 1 L1 128->128 | 2 L2 136->120 | 3 L3 120->64 | 4 P0|CMP 128->64|24 | 5 P1 64->64
-//          (biases as K rows, two-term weights W_hi + W_lo; tensor-memory placement: geo_dcol)
-//   colour 12 RE1 16->35 R0->R1 | 6 BASE0 105->64 R0->R1 | 7 BASE1 64->32 R1->R0 | 8 VIS1A 32->32 R0->R1 | 9 VIS1B 32->33 R1->R0
-//          10 VIS2A 32->32 R0->R1 | 11 OUT0 37->16 R1->R0     (R0/R1: the slot's two 64-column regions, in-place epilogues)
+//   colour 12 RE1 16->35 | 6 BASE0 105->64 | 7 BASE1 64->32 | 8 VIS1A 32->32 | 9 VIS1B 32->33 | 10 VIS2A 32->32 | 11 OUT0 37->16
 #include <atomic>
 #include <cstdlib>
 #include <type_traits>
@@ -34,13 +31,10 @@
 namespace kpn {
 namespace {
 
-constexpr int ROW_WARPS = 4;
-constexpr int NSLOT = 2;                                  // geo kernel tile slots
-constexpr int CSLOT = 4;                                  // colour kernel tile slots (4 x 128 TMEM columns)
-constexpr int TCC_THREADS = CSLOT * ROW_WARPS * 32;       // 512: 16 row warps, row warp 0 of a slot issues its MMAs
-constexpr int GEO_NSTAGE = 6;   // colour kernel: RE1 (stage 12), then stages 6..11
+constexpr int ROW_WARPS = 4;                              // warps of a warpgroup
+constexpr int GEO_NSTAGE = 6;                             // colour stages start at plan.st[6]
 constexpr int SPW = 10;                                   // samples per warp (3 views each)
-constexpr int SPT = SPW * ROW_WARPS;                      // samples per tile
+constexpr int SPT = SPW * ROW_WARPS;                      // samples per colour tile (128 rows)
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr unsigned FULL = 0xffffffffu;
 
@@ -100,63 +94,6 @@ __device__ __forceinline__ float boundary_weight_fast(const Proj& q) {
   return w;
 }
 
-struct RowCtx {
-  uint32_t R0, R1;      // TMEM addresses (lane field already set) of the slot's two column regions
-  uint64_t* a_ready;    // row warps -> MMA issuer : "layer input is in TMEM"   (one arrival per row warp)
-  uint64_t* acc_ready;  // MMA issuer -> row threads : "accumulator is complete"  (tcgen05.commit)
-  uint32_t ph;          // parity of acc_ready this thread waits on next
-  int gb;               // first lane of this row's 3-view group
-  int l1, l2;           // the other two lanes of the group
-  int issuer;           // this warp issues the slot's MMAs (row warp 0 of the slot); no dedicated issuer warp
-  uint32_t pha;         // parity of a_ready the issuer waits on next
-  uint32_t slot_tm, wlo0, el;
-};
-
-// The activation tile lives in tensor memory: tcgen05.wait::st + tcgen05.fence::before_thread_sync order it, so the arrive
-// itself carries no release (a release would also drain the thread's unrelated global loads).
-__device__ __forceinline__ void signal_a(RowCtx& c) {
-  tc::wait_st();
-  tc::fence_before_sync();
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0)
-    asm volatile("mbarrier.arrive.relaxed.cta.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(c.a_ready)) : "memory");
-}
-__device__ __forceinline__ void wait_acc(RowCtx& c) {
-  tc::mbar_wait(c.acc_ready, c.ph, 0x20u);
-  c.ph ^= 1u;
-  tc::fence_after_sync();
-}
-__device__ __forceinline__ float gsum(const RowCtx& c, float x) {
-  return x + __shfl_sync(FULL, x, c.l1) + __shfl_sync(FULL, x, c.l2);
-}
-__device__ __forceinline__ float gmin(const RowCtx& c, float x) {
-  return fminf(x, fminf(__shfl_sync(FULL, x, c.l1), __shfl_sync(FULL, x, c.l2)));
-}
-__device__ __forceinline__ float gmax(const RowCtx& c, float x) {
-  return fmaxf(x, fmaxf(__shfl_sync(FULL, x, c.l1), __shfl_sync(FULL, x, c.l2)));
-}
-
-// acc (NCH*32 fp32 columns at src) -> act(acc + bias) as packed fp16 at dst (in place allowed: dst <= src).
-template <int NCH, int ACT>  // ACT 1 = softplus100, 2 = ELU
-__device__ __forceinline__ void epi_inplace(uint32_t src, uint32_t dst, const float* __restrict__ bias) {
-  uint32_t r[2][32];
-  tc::tmem_ld32(src, r[0]);
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    tc::wait_ld();
-    if (ch + 1 < NCH) tc::tmem_ld32(src + (ch + 1) * 32, r[(ch + 1) & 1]);   // next chunk in flight while this one is processed
-    uint32_t o[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float x0 = u2f(r[ch & 1][2 * i]) + bias[ch * 32 + 2 * i], x1 = u2f(r[ch & 1][2 * i + 1]) + bias[ch * 32 + 2 * i + 1];
-      if (ACT == 1) { x0 = sp_fast(x0); x1 = sp_fast(x1); }
-      else { x0 = elu_fast(x0); x1 = elu_fast(x1); }
-      o[i] = tc::pack_h2(x0, x1);
-    }
-    tc::tmem_st16(dst + ch * 16, o);
-  }
-}
-
 // Keypoint encoding of one keypoint with sp_level == 3: sin/cos(pi*2^l*dz) from one sincos + double angles.
 __device__ __forceinline__ void encode_fast(const SceneS& S, int v, int k, const float c[3], float e[7]) {
   const float4 kc = S.kc[v][k];
@@ -173,87 +110,7 @@ __device__ __forceinline__ void encode_fast(const SceneS& S, int v, int k, const
   e[0] = dz * w; e[1] = s * w; e[2] = co * w; e[3] = s2 * w; e[4] = c2 * w; e[5] = s4 * w; e[6] = c4 * w;
 }
 
-// =====================================================================================================================
-// geometry + density pass: two threads per row (column halves h = 0/1 in different warps of the same TMEM lane quarter)
-// =====================================================================================================================
-// Tensor-memory columns of one slot (256): the activation tile A (packed fp16 pairs) always starts at column 0, the fp32
-// accumulator D of a stage sits at geo_dcol(stage); a stage's A is rebuilt while the previous stage's D is being read.
-//   stage  A columns                                                           D columns
-//   0 L0   [0,K0P/2): thread 0 run | thread 1 run (tc_kmap)                      [128,256)
-//   1 L1   [0,64) act | [64,72) bias chunk                                       [128,256)
-//   2 L2   [0,64) act | [64,68) feat8 | 68 bias | [69,72) 0                      [128,256)
-//   3 L3   [0,60) act | 60 bias | [61,64) 0                                      [192,256)
-//   4 P0|C [0,32) mean hi | [32,64) var hi | [64,96) mean lo | [96,128) var lo | [128,136) bias chunk    [160,256)
-//   5 P1   [0,32) act hi | [32,64) act lo | [64,72) bias chunk                   [128,192)
-__host__ __device__ constexpr int geo_dcol(int stage) { return stage == 3 ? 192 : stage == 4 ? 160 : 128; }
-
 constexpr uint32_t H2_ONE = 0x00003C00u;   // fp16 pair (1.0, 0.0): the activation column that multiplies the bias row
-
-#ifdef KPN_STAGE_TIMING
-// Instrumented build only (tools/stage_times.py): cycle stamps of one issuer warp (block 0, slot 0), per tile:
-// [0] tile start, [1] stage-0 input built, then per stage s: [2+5s] own arrive done, [3+5s] every row warp of the pair has
-// arrived, [4+5s] MMAs issued + committed, [5+5s] accumulator complete (this warp woke up), [6+5s] epilogue done.
-constexpr int TIM_TILES = 48, TIM_WORDS = 32;
-__device__ unsigned long long kpn_tim[3 * TIM_TILES * TIM_WORDS + 256];   // (+ 256: cycles every block of the view-sequential kernel took)   // rows [0, TIM_TILES): the issuer warp (h = 0); then its h = 1 partner
-                                                                     // (view-sequential kernel: row warp 0, issuer, producer warp 0)
-__device__ int kpn_tim_tile[2];   // tiles each of the two warps has recorded
-#define TIM(idx) do { if (tim_on && lane == 0) kpn_tim[tim_row * TIM_WORDS + (idx)] = clock64(); } while (0)
-#else
-#define TIM(idx) do { } while (0)
-#endif
-
-// (what the h = 1 thread of a row hands to its h = 0 partner at the end of a tile: g0, rad partial sums + 6 latent words)
-
-struct GeoCtx {
-  uint32_t tm;          // TMEM address of the slot with this warp's lane quarter
-  uint32_t a_ready_cl;  // cluster-mapped shared address of the LEADER CTA's a_ready barrier of this slot
-  uint64_t* acc_ready;  // this CTA's copy of the slot's accumulator barrier
-  uint32_t ph;
-  int l1, l2;           // the other two lanes of this row's 3-view group
-  // the slot's MMA issuer (one row warp of the pair's leader CTA; there is no dedicated control warp, so that 16 warps keep
-  // 128 registers per thread): waits for the slot's a_ready phase, issues the stage's MMAs, commits to acc_ready
-  int issuer;
-  uint64_t* a_ready;    // leader CTA's barrier (local address, issuer only)
-  uint32_t pha;
-  uint32_t slot_tm, wlo0, lod, el;
-  int lo_mask;
-  int relaxed;          // arrive without release semantics (default; KPN_RELAXED_ARRIVE=0 reverts): the activation tile lives in
-                        // tensor memory and is ordered by tcgen05.wait::st + tcgen05.fence::before_thread_sync; a release
-                        // would additionally drain the row's in-flight prefetch loads (measured: 40.4 -> 35.4 ms/frame)
-};
-
-__device__ __forceinline__ void geo_signal(const GeoCtx& c, int lane) {
-  tc::wait_st();
-  tc::fence_before_sync();
-  __syncwarp();
-  if (lane == 0) {
-    if (c.relaxed) asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(c.a_ready_cl) : "memory");
-    else asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(c.a_ready_cl) : "memory");
-  }
-}
-__device__ __forceinline__ void geo_wait(GeoCtx& c) {
-  tc::mbar_wait(c.acc_ready, c.ph, 0x100u);
-  c.ph ^= 1u;
-  tc::fence_after_sync();
-}
-template <int NK, int STAGE>
-__device__ __forceinline__ void geo_issue(uint32_t slot_tm, uint32_t d_tm, uint32_t wlo0, uint32_t lo_delta, int lo_mask, uint32_t el);
-// issuer warp only: once every row warp of the pair has signalled this stage's input, issue its MMAs
-template <int NK, int STAGE>
-__device__ __forceinline__ void geo_mma(GeoCtx& c, bool tim_on = false, int tim_row = 0, int lane = 0) {
-  if (c.issuer) {
-    tc::mbar_wait(c.a_ready, c.pha, 0x10u + (uint32_t)STAGE);
-    c.pha ^= 1u;
-    tc::fence_after_sync();
-    TIM(3 + 5 * STAGE);
-    geo_issue<NK, STAGE>(c.slot_tm, c.slot_tm + (uint32_t)geo_dcol(STAGE), c.wlo0, c.lod, c.lo_mask, c.el);
-    tc::mma_commit2_el(c.acc_ready, c.el);
-    TIM(4 + 5 * STAGE);
-  }
-}
-__device__ __forceinline__ float gsum(const GeoCtx& c, float x) {
-  return x + __shfl_sync(FULL, x, c.l1) + __shfl_sync(FULL, x, c.l2);
-}
 
 // softplus(beta=100) of two accumulators -> packed fp16 pair, on packed halves and WITHOUT the special-function unit: x is
 // rounded to fp16 first (the result is an fp16 activation anyway), y = max(x,0) + c(|x|) with the correction
@@ -280,450 +137,25 @@ __device__ __forceinline__ uint32_t sp_pair(uint32_t a0, uint32_t a1) {
   return *reinterpret_cast<const uint32_t*>(&y);
 }
 
-__device__ __forceinline__ uint32_t sel3(int v, uint32_t a, uint32_t b, uint32_t c) { return v == 0 ? a : (v == 1 ? b : c); }
-
-// store N registers to consecutive tensor-memory columns starting at column C0 (relative alignment known at compile time)
-template <int N, int C0>
-__device__ __forceinline__ void st_cols(uint32_t addr, const uint32_t* r) {
-  if constexpr (N >= 32 && C0 % 32 == 0) { tc::tmem_st32(addr, r); st_cols<N - 32, C0 + 32>(addr + 32, r + 32); }
-  else if constexpr (N >= 16 && C0 % 16 == 0) { tc::tmem_st16(addr, r); st_cols<N - 16, C0 + 16>(addr + 16, r + 16); }
-  else if constexpr (N >= 8 && C0 % 8 == 0) { tc::tmem_st8(addr, r); st_cols<N - 8, C0 + 8>(addr + 8, r + 8); }
-  else static_assert(N == 0, "run is not a multiple of 8 columns");
-}
-
-// epilogue of a 128-wide softplus stage: this thread's 64 accumulator columns at d -> 32 packed columns at a.
-// bias_tail: the last 4 packed columns become (1,0),0,0,0 (layer-3 input: bias column + K padding).
-__device__ __forceinline__ void geo_epi_sp(uint32_t d, uint32_t a, bool bias_tail) {
-  uint32_t r[64];
-  tc::tmem_ld32(d, r);
-  tc::tmem_ld32(d + 32, r + 32);
-  tc::wait_ld();
-  uint32_t o[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) o[i] = sp_pair(r[2 * i], r[2 * i + 1]);
-  tc::tmem_st16(a, o);
-#pragma unroll
-  for (int i = 0; i < 16; ++i) o[i] = sp_pair(r[32 + 2 * i], r[33 + 2 * i]);
-  if (bias_tail) { o[12] = H2_ONE; o[13] = 0u; o[14] = 0u; o[15] = 0u; }
-  tc::tmem_st16(a + 16, o);
-}
-
-// Gather staging (PREF): while a tile's layer-0 MMAs run, each row thread gathers the source-view features of its row of the
-// slot's NEXT tile (the long-latency part of the stage-0 input) into shared memory as packed fp16 pairs; the next tile's build
-// only copies them into tensor memory.  Words per row: 32 feat64 (thread 0 owns [0, FA/2), thread 1 the rest) + 4 feat8 (a
-// tile consumes its feat8 words after stage 1, the next tile's are staged after stage 4: one buffer is enough).  Word w of row
-// r sits at [w * 128 + r] so that a warp's accesses are conflict free.  2 slots x 36 words x 128 rows = 36 KB, which fits
-// behind the resident weights for both keypoint counts (18: 173 KB, 24: 185 KB per CTA).
-constexpr int GEO_FW = 36;
-__host__ __device__ constexpr bool geo_pref(int n_kpt) { return n_kpt == 18 || n_kpt == 24; }
-struct GeoPre { int id; float p[3]; };   // the sample this row shades in the slot's next tile
-
-// Asynchronous halves of a bilinear gather: issue the 4 tap loads of float4 groups [g0, g0 + NG) of a channel-last map now,
-// blend + pack + stage them after the next accumulator wait (the loads fly while the tensor core works).
-template <int NG>
-__device__ __forceinline__ void taps_issue(const MapDesc& m, int v, const Taps& t, int g0, float4 (&r)[2][4]) {
-  const int c4 = m.C >> 2;
-  const float4* base = (const float4*)m.ptr + (size_t)v * m.H * m.W * c4 + g0;
-  const float4* p00 = base + (size_t)t.o00 * c4;
-  const float4* p01 = base + (size_t)t.o01 * c4;
-  const float4* p10 = base + (size_t)t.o10 * c4;
-  const float4* p11 = base + (size_t)t.o11 * c4;
-#pragma unroll
-  for (int i = 0; i < NG; ++i) { r[i][0] = __ldg(p00 + i); r[i][1] = __ldg(p01 + i); r[i][2] = __ldg(p10 + i); r[i][3] = __ldg(p11 + i); }
-}
-template <int NG>
-__device__ __forceinline__ void taps_stage(const float (&w)[4], const float4 (&r)[2][4], uint32_t* __restrict__ fb, int word0) {
-#pragma unroll
-  for (int i = 0; i < NG; ++i) {
-    const float4 a = r[i][0], b = r[i][1], c = r[i][2], d = r[i][3];
-    const float f0 = a.x * w[0] + b.x * w[1] + c.x * w[2] + d.x * w[3], f1 = a.y * w[0] + b.y * w[1] + c.y * w[2] + d.y * w[3];
-    const float f2 = a.z * w[0] + b.z * w[1] + c.z * w[2] + d.z * w[3], f3 = a.w * w[0] + b.w * w[1] + c.w * w[2] + d.w * w[3];
-    fb[(word0 + 2 * i) * 128] = tc::pack_h2(f0, f1);
-    fb[(word0 + 2 * i + 1) * 128] = tc::pack_h2(f2, f3);
+__device__ __forceinline__ void stage_scene(SceneS& scs, const DevScene& g, int NK, int t, int nthreads) {
+  for (int i = t; i < 3 * 12; i += nthreads) { scs.P[i / 12][i % 12] = g.P[i / 12][i % 12]; scs.E[i / 12][i % 12] = g.E[i / 12][i % 12]; }
+  for (int i = t; i < 3 * 3; i += nthreads) scs.C[i / 3][i % 3] = g.C[i / 3][i % 3];
+  for (int i = t; i < 3 * NK; i += nthreads)
+    scs.kc[i / NK][i % NK] = make_float4(g.kc[i / NK][i % NK][0], g.kc[i / NK][i % NK][1], g.kc[i / NK][i % NK][2], 0.0f);
+  if (t == 0) {
+    scs.wm1 = g.wm1; scs.hm1 = g.hm1; scs.znear = g.znear; scs.inv_zrange = 1.0f / (g.zfar - g.znear);
+    scs.sp_scale = g.sp_scale; scs.inv2sig2 = g.inv2sig2; scs.inv_wm1 = 1.0f / g.wm1; scs.inv_hm1 = 1.0f / g.hm1;
+    scs.f64 = g.f64; scs.f8 = g.f8; scs.ftex = g.ftex; scs.img = g.img;
   }
 }
 
-template <int NK>
-__device__ __forceinline__ void geo_prefetch(const SceneS& sc, const SampleSrc& src, const int* __restrict__ list, int count, int tile,
-                                             int q4, int h, int lane, uint32_t* __restrict__ fb, int parity, GeoPre& pre) {
-  constexpr int FA = tc_l0_fa(NK);
-  const int g = lane / 3;
-  const int v = lane - 3 * g;
-  const int si = tile * SPT + q4 * SPW + min(g, SPW - 1);
-  pre.id = list[max(min(si, count - 1), 0)];
-  float d[3];
-  fetch_sample(src, pre.id, pre.p, d);
-  const Proj q = project_s(sc, v, pre.p);
-  const Taps t64 = make_taps(q.u, q.v, sc.f64.W, sc.f64.H);
-  if (h == 0) {
-#pragma unroll
-    for (int gq = 0; gq < FA / 4; ++gq) {
-      float f[4];
-      gather_f32<1>(sc.f64, v, t64, gq, f);
-      fb[(2 * gq) * 128] = tc::pack_h2(f[0], f[1]);
-      fb[(2 * gq + 1) * 128] = tc::pack_h2(f[2], f[3]);
-    }
-  } else {
-#pragma unroll
-    for (int gq = FA / 4; gq < 16; ++gq) {
-      float f[4];
-      gather_f32<1>(sc.f64, v, t64, gq, f);
-      fb[(2 * gq) * 128] = tc::pack_h2(f[0], f[1]);
-      fb[(2 * gq + 1) * 128] = tc::pack_h2(f[2], f[3]);
-    }
-    const Taps t8 = make_taps(q.u, q.v, sc.f8.W, sc.f8.H);
-    float g8[8];
-    gather_f32<2>(sc.f8, v, t8, 0, g8);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) fb[(32 + i) * 128] = tc::pack_h2(g8[2 * i], g8[2 * i + 1]);
+__device__ __forceinline__ void load_weights(uint8_t* dst, const uint8_t* src, uint32_t bytes, uint64_t* wbar) {
+  tc::mbar_expect_tx(wbar, bytes);
+  for (uint32_t off = 0; off < bytes; off += 32768u) {
+    uint32_t n = bytes - off < 32768u ? bytes - off : 32768u;
+    tc::bulk_g2s(dst + off, src + off, n, wbar);
   }
-}
-
-// One tile of the geometry pass.  PREF: `pre` holds this tile's sample on entry (its gathers are staged in `fb`) and the next
-// tile's on exit, `nid` the sample id of the next tile on entry and of the tile after that (`next2_tile`) on exit;
-// `next_tile` < 0: nothing to prefetch.
-template <int NK, bool PREF>
-__device__ __forceinline__ void geo_tile(const SceneS& sc, const float* __restrict__ wp2,
-                                         const SampleSrc& src, const int* __restrict__ list, int count, int tile, int next_tile,
-                                         int next2_tile, int& nid, uint32_t* __restrict__ fb, int parity, GeoPre& pre, GeoCtx& cx,
-                                         int q4, int h, int lane, int bar_id, int query_mode, const ShadeOut& so,
-                                         uint4* __restrict__ lat_out) {
-  constexpr int NP = NK / 2, PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
-  const uint32_t A = cx.tm;
-#ifdef KPN_STAGE_TIMING
-  const bool tim_on = blockIdx.x == 0 && bar_id == 1 && kpn_tim_tile[h] < TIM_TILES;   // slot 0, lane quarter 0 of the leader CTA
-  const int tim_row = tim_on ? h * TIM_TILES + kpn_tim_tile[h] : 0;
-#else
-  constexpr bool tim_on = false;
-  constexpr int tim_row = 0;
-#endif
-  TIM(0);
-  const int g = lane / 3;
-  const int v = lane - 3 * g;           // lanes 30,31 replay views 0,1 of the warp's last sample (results unused)
-  const int si = tile * SPT + q4 * SPW + min(g, SPW - 1);
-  const bool writer = (h == 0) && (lane < 3 * SPW) && (v == 0) && (si < count);
-  int id;
-  float p[3];
-  if (PREF) {
-    id = pre.id; p[0] = pre.p[0]; p[1] = pre.p[1]; p[2] = pre.p[2];
-  } else {
-    float d[3];
-    id = list[min(si, count - 1)];
-    fetch_sample(src, id, p, d);
-  }
-  const Proj q = project_s(sc, v, p);
-  const float bw = boundary_weight_fast(q);
-  const float pw = bw / (gsum(cx, bw) + 1e-6f);  // reference src/model.py:750-759 (mask == 1 for shaded samples)
-
-  // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap
-  {
-    float c[3];
-    {
-      const float* E = sc.E[v];
-      c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
-      c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
-      c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
-    }
-    Taps t64;
-    if (!PREF) t64 = make_taps(q.u, q.v, sc.f64.W, sc.f64.H);
-    if (h == 0) {
-      constexpr int N0 = 7 * PA + FA / 2;
-      uint32_t a[N0];
-      if (PREF) {
-#pragma unroll
-        for (int i = 0; i < FA / 2; ++i) a[7 * PA + i] = fb[i * 128];
-      } else {
-#pragma unroll
-        for (int gq = 0; gq < FA / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(sc.f64, v, t64, gq, f);
-          a[7 * PA + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[7 * PA + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < PA; ++j) {
-        float e0[7], e1[7];
-        encode_fast(sc, v, 2 * j, c, e0);
-        encode_fast(sc, v, 2 * j + 1, c, e1);
-#pragma unroll
-        for (int r = 0; r < 7; ++r) a[7 * j + r] = tc::pack_h2(e0[r], e1[r]);
-      }
-      st_cols<N0, 0>(A, a);
-    } else {
-      constexpr int C1 = 7 * PA + FA / 2;           // first column of this thread's run
-      constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
-      constexpr int N1 = tc_k0p(NK) / 2 - C1;
-      uint32_t a[N1];
-      if (PREF) {
-#pragma unroll
-        for (int i = 0; i < NF; ++i) a[NE + i] = fb[(FA / 2 + i) * 128];
-      } else {
-#pragma unroll
-        for (int gq = 0; gq < (64 - FA) / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(sc.f64, v, t64, FA / 4 + gq, f);
-          a[NE + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[NE + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
-        }
-      }
-#pragma unroll
-      for (int j = PA; j < NP; ++j) {
-        float e0[7], e1[7];
-        encode_fast(sc, v, 2 * j, c, e0);
-        encode_fast(sc, v, 2 * j + 1, c, e1);
-#pragma unroll
-        for (int r = 0; r < 7; ++r) a[7 * (j - PA) + r] = tc::pack_h2(e0[r], e1[r]);
-      }
-      a[NE + NF] = H2_ONE;
-#pragma unroll
-      for (int i = NE + NF + 1; i < N1; ++i) a[i] = 0u;
-      st_cols<N1, C1>(A + C1, a);
-    }
-  }
-  // ---- staging of this row's NEXT tile, spread over the six accumulator waits of this tile: every global load is issued
-  //      just before a stage is signalled and consumed right after that stage's accumulator arrived, so its latency hides
-  //      behind the tensor core instead of stalling the row (each thread stages only the words it will read itself).
-  const bool pf = PREF && next_tile >= 0;
-  constexpr int FG = FA / 4;                 // feat64 float4 groups owned by thread 0 (thread 1: [FG, 16) + the two feat8 groups)
-  static_assert(!PREF || FG == 10, "the window plan below assumes 10 | 6 feat64 groups per thread (18 keypoints)");
-  float4 pr[2][4];
-  float pwt[4];
-  float nu = 0.0f, nv = 0.0f;
-  // windows 1..5: feature gathers of the next tile, two float4 groups each (thread 0: feat64 groups 2w, 2w+1; thread 1: feat64
-  // groups 10+2w, 11+2w for w < 3, then the two feat8 groups)
-  auto win_issue = [&](int w) {
-    if (h == 1 && w == 4) return;
-    const bool f8w = (h == 1) && (w == 3);
-    const MapDesc& m = f8w ? sc.f8 : sc.f64;
-    const Taps t = make_taps(nu, nv, m.W, m.H);   // recomputed per window: holding the taps across the tile costs more (registers)
-    pwt[0] = t.w00; pwt[1] = t.w01; pwt[2] = t.w10; pwt[3] = t.w11;
-    taps_issue<2>(m, v, t, f8w ? 0 : (h == 0 ? 2 * w : FG + 2 * w), pr);
-  };
-  auto win_stage = [&](int w) {
-    if (h == 1 && w == 4) return;
-    taps_stage<2>(pwt, pr, fb, h == 0 ? 4 * w : (w == 3 ? 32 : 2 * FG + 4 * w));
-  };
-  TIM(1);
-  geo_signal(cx, lane);
-  TIM(2);
-  // window 0: position of the next tile's sample (its id was fetched during the previous tile; reference src/model.py:1057:
-  // p = cam_pos + dir * z, or an explicit query point) and the id of the tile after that
-  float nl[7];
-  int nid2 = 0;
-  if (pf) {
-    if (src.mode == 0) {
-      const int r = nid / src.S;
-      nl[0] = src.z ? __ldg(src.z + nid) : coarse_depth(__ldg(src.ray_nf + 2 * r), __ldg(src.ray_nf + 2 * r + 1), nid - r * src.S, src.S);
-      nl[1] = __ldg(src.ray_d + 3 * r); nl[2] = __ldg(src.ray_d + 3 * r + 1); nl[3] = __ldg(src.ray_d + 3 * r + 2);
-      nl[4] = __ldg(src.o); nl[5] = __ldg(src.o + 1); nl[6] = __ldg(src.o + 2);
-    } else {
-      nl[0] = __ldg(src.pts + 3ll * nid); nl[1] = __ldg(src.pts + 3ll * nid + 1); nl[2] = __ldg(src.pts + 3ll * nid + 2);
-    }
-    if (next2_tile >= 0) nid2 = __ldg(list + max(min(next2_tile * SPT + q4 * SPW + min(g, SPW - 1), count - 1), 0));
-  }
-  const uint32_t dh = A + 128u + 64u * (uint32_t)h, ah = A + 32u * (uint32_t)h;
-  // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720); thread 0 writes the bias chunk, thread 1 the feat8 | bias chunk
-  geo_mma<NK, 0>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(5);
-  if (pf) {
-    pre.id = nid;
-    if (src.mode == 0) { pre.p[0] = nl[4] + nl[1] * nl[0]; pre.p[1] = nl[5] + nl[2] * nl[0]; pre.p[2] = nl[6] + nl[3] * nl[0]; }
-    else { pre.p[0] = nl[0]; pre.p[1] = nl[1]; pre.p[2] = nl[2]; }
-    const Proj nq = project_s(sc, v, pre.p);
-    nu = nq.u; nv = nq.v;
-    nid = nid2;
-  }
-  geo_epi_sp(dh, ah, false);
-  if (h == 0) {
-    const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-    tc::tmem_st8(A + 64, b);
-  }
-  TIM(6);
-  geo_signal(cx, lane);
-  TIM(7);
-  if (pf) win_issue(0);
-  geo_mma<NK, 1>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(10);
-  if (pf) win_stage(0);
-  geo_epi_sp(dh, ah, false);
-  if (h == 1) {
-    uint32_t b[8] = {0u, 0u, 0u, 0u, H2_ONE, 0u, 0u, 0u};
-    if (PREF) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) b[i] = fb[(32 + i) * 128];
-    } else {
-      const Taps t8 = make_taps(q.u, q.v, sc.f8.W, sc.f8.H);
-      float g8[8];
-      gather_f32<2>(sc.f8, v, t8, 0, g8);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) b[i] = tc::pack_h2(g8[2 * i], g8[2 * i + 1]);
-    }
-    tc::tmem_st8(A + 64, b);
-  }
-  TIM(11);
-  geo_signal(cx, lane);
-  TIM(12);
-  if (pf) win_issue(1);
-  geo_mma<NK, 2>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(15);
-  if (pf) win_stage(1);
-  geo_epi_sp(dh, ah, h == 1);
-  TIM(16);
-  geo_signal(cx, lane);
-  TIM(17);
-  if (pf) win_issue(2);
-  // ---- view pooling: weighted mean || variance over the 3 lanes of the group (src/utils.py:722-748); this thread owns 32
-  //      of the 64 feature columns; the density tail's inputs are kept to two fp16 terms (hi | lo)
-  geo_mma<NK, 3>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(20);
-  if (pf) win_stage(2);
-  {
-    uint32_t r[32];
-    tc::tmem_ld32(A + 192u + 32u * (uint32_t)h, r);
-    tc::wait_ld();
-#pragma unroll
-    for (int cb = 0; cb < 2; ++cb) {
-      uint32_t mh[8], vh[8], ml[8], vl[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float x0 = u2f(r[16 * cb + 2 * i]), x1 = u2f(r[16 * cb + 2 * i + 1]);
-        const float m0 = gsum(cx, pw * x0), m1 = gsum(cx, pw * x1);
-        const float d0 = x0 - m0, d1 = x1 - m1;
-        const float v0 = gsum(cx, pw * d0 * d0), v1 = gsum(cx, pw * d1 * d1);
-        split_h2(m0, m1, mh[i], ml[i]);
-        split_h2(v0, v1, vh[i], vl[i]);
-      }
-      const uint32_t col = A + 16u * (uint32_t)h + 8u * (uint32_t)cb;
-      tc::tmem_st8(col, mh);
-      tc::tmem_st8(col + 32, vh);
-      tc::tmem_st8(col + 64, ml);
-      tc::tmem_st8(col + 96, vl);
-    }
-    if (h == 0) {
-      const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-      tc::tmem_st8(A + 128, b);
-    }
-  }
-  TIM(21);
-  geo_signal(cx, lane);
-  TIM(22);
-  if (pf) win_issue(3);
-  // ---- P0 (softplus, two fp16 terms out) | compress (linear; this thread keeps 12 of the 24 latent values as 6 fp16 pairs)
-  geo_mma<NK, 4>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(25);
-  if (pf) win_stage(3);
-  uint32_t latp[6];
-  {
-    uint32_t rc[16], r[32];
-    tc::tmem_ld8(A + 160u + 64u + 8u * (uint32_t)h, rc);        // h = 0: latent 0..15, h = 1: latent 8..23 (two naturally
-    tc::tmem_ld8(A + 160u + 72u + 8u * (uint32_t)h, rc + 8);    // aligned 8-column loads)
-    tc::tmem_ld32(A + 160u + 32u * (uint32_t)h, r);
-    tc::wait_ld();
-#pragma unroll
-    for (int i = 0; i < 6; ++i) {
-      const float l0 = u2f(h ? rc[4 + 2 * i] : rc[2 * i]), l1 = u2f(h ? rc[5 + 2 * i] : rc[2 * i + 1]);
-      latp[i] = tc::pack_h2(l0, l1);
-    }
-    // The three view rows of a sample hold the same pooled input, hence (to fp32 rounding) the same accumulator row: lane v
-    // activates only the column pairs j = 3k + v of its own row and the group all-gathers the packed results by shuffle.
-    uint32_t hk[6], lk[6];
-#pragma unroll
-    for (int k = 0; k < 6; ++k) {   // k = 5: only pair 15 exists; lanes with v > 0 recompute it, nobody reads their copy
-      const int j0 = 3 * k, j1 = min(3 * k + 1, 15), j2 = min(3 * k + 2, 15);
-      const float x0 = u2f(sel3(v, r[2 * j0], r[2 * j1], r[2 * j2])), x1 = u2f(sel3(v, r[2 * j0 + 1], r[2 * j1 + 1], r[2 * j2 + 1]));
-      split_h2(sp_fast(x0), sp_fast(x1), hk[k], lk[k]);
-    }
-    uint32_t hi[16], lo[16];
-    const int gb = lane - v;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      hi[j] = __shfl_sync(FULL, hk[j / 3], gb + j % 3);
-      lo[j] = __shfl_sync(FULL, lk[j / 3], gb + j % 3);
-    }
-    tc::tmem_st16(A + 16u * (uint32_t)h, hi);
-    tc::tmem_st16(A + 32u + 16u * (uint32_t)h, lo);
-    if (h == 0) {
-      const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-      tc::tmem_st8(A + 64, b);
-    }
-  }
-  TIM(26);
-  geo_signal(cx, lane);
-  TIM(27);
-  if (pf) win_issue(4);
-  // ---- P1 (softplus) then the 64->2 density head in fp32 on the CUDA cores: each thread a partial dot over its 32 columns
-  geo_mma<NK, 5>(cx, tim_on, tim_row, lane);
-  geo_wait(cx);
-  TIM(30);
-  if (pf) win_stage(4);
-  float g0 = 0.0f, rad = 0.0f;
-  {
-    uint32_t r[32];
-    tc::tmem_ld32(A + 128u + 32u * (uint32_t)h, r);
-    tc::wait_ld();
-    // same split over the three lanes of the group: lane v takes columns 3k + v of its 32, the partial dots are group sums
-    const float* w0 = wp2 + 32 * h + v;
-#pragma unroll
-    for (int k = 0; k < 11; ++k) {
-      const int c0 = 3 * k, c1 = min(3 * k + 1, 31), c2 = min(3 * k + 2, 31);
-      const float hh = sp_fast(u2f(sel3(v, r[c0], r[c1], r[c2])));
-      const bool live = 3 * k + v < 32;   // k = 10: columns 30 and 31 exist, 32 does not
-      const float a0 = live ? w0[3 * k] : 0.0f, a1 = live ? w0[64 + 3 * k] : 0.0f;
-      g0 = fmaf(a0, hh, g0);
-      rad = fmaf(a1, hh, rad);
-    }
-    g0 = gsum(cx, g0);
-    rad = gsum(cx, rad);
-  }
-  // ---- the h = 1 thread hands its partial sums and latent half to its partner (same row = same tensor-memory lane, other warp)
-  //      through 8 tensor-memory columns of that lane: the activation region is dead once the P1 accumulator has arrived, and
-  //      columns [0, 8) belong to the partner's own stage-0 run, which it only rebuilds after it has read them
-  TIM(31);
-#ifdef KPN_STAGE_TIMING
-  if (tim_on && lane == 0) kpn_tim_tile[h] = tim_row - h * TIM_TILES + 1;
-#endif
-  if (h == 1) {
-    const uint32_t xw[8] = {__float_as_uint(g0), __float_as_uint(rad), latp[0], latp[1], latp[2], latp[3], latp[4], latp[5]};
-    tc::tmem_st8(A, xw);
-    tc::wait_st();
-    tc::fence_before_sync();
-    tc::named_arrive(bar_id, 64);
-    return;
-  }
-  tc::named_sync(bar_id, 64);
-  tc::fence_after_sync();
-  uint32_t xr[8];
-  tc::tmem_ld8(A, xr);
-  tc::wait_ld();
-  const uint4 x0 = make_uint4(xr[0], xr[1], xr[2], xr[3]), x1 = make_uint4(xr[4], xr[5], xr[6], xr[7]);
-  g0 += __uint_as_float(x0.x) + wp2[128];
-  rad += __uint_as_float(x0.y) + wp2[129];
-  // ---- outputs of the geometry pass: alpha / sdf (eval_func, src/model.py:978-997) and, where a colour will be needed
-  //      (density > 0: a sample with alpha == 0 composites with weight exactly 0, skipping its colour is exact; every valid
-  //      sample in query mode), the compressed latent at the sample's own list index.  The colour work list is built from the
-  //      alpha records by colour_list_kernel afterwards: no atomic round trip sits in this kernel's tile loop.
-  {
-    const bool need = writer && (query_mode != 0 || rad > 0.0f);
-    if (writer) {
-      if (query_mode) {
-        float* o = so.out5 + 5ll * id;
-        o[0] = g0; o[1] = rad; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f;
-      } else {
-        so.ao[so.list_base + si] = make_float2(fmaxf(rad, 0.0f), g0);   // compact record at the sample's absolute list position
-      }
-    }
-    if (need) {
-      lat_out[3ll * si + 0] = make_uint4(latp[0], latp[1], latp[2], latp[3]);
-      lat_out[3ll * si + 1] = make_uint4(latp[4], latp[5], x0.z, x0.w);
-      lat_out[3ll * si + 2] = x1;
-    }
-  }
+  tc::mbar_wait(wbar, 0, 0x30u);
 }
 
 // Colour work list: the entries of the first list whose sample needs a colour (alpha > 0), in list order, as (index into the
@@ -766,19 +198,429 @@ colour_list_kernel(const int* __restrict__ list, const int* __restrict__ count_p
   }
 }
 
-// Colour pass for one tile of the second work list (entries: x = slot of the latent in the scratch buffer, y = sample id).
-template <int NK, int STAGE>
-__device__ __forceinline__ void col_mma(RowCtx& c);
+// =====================================================================================================================
+// activation tiles, warpgroup synchronisation
+// =====================================================================================================================
+// store N words (packed fp16 pairs) of row r at word columns [c0, c0 + N) of an activation tile; c0 % 4 == 0
+template <int ROWS, int N>
+__device__ __forceinline__ void a_put(uint8_t* tile, int r, int c0, const uint32_t* w) {
+  static_assert(N % 4 == 0, "runs are whole 16-byte chunks");
+#pragma unroll
+  for (int i = 0; i < N; i += 4)
+    *reinterpret_cast<uint4*>(tile + tc::a_word_off<ROWS>(r, c0 + i)) = make_uint4(w[i], w[i + 1], w[i + 2], w[i + 3]);
+}
+__device__ __forceinline__ void a_word(uint8_t* tile64, int r, int c, uint32_t w) {
+  *reinterpret_cast<uint32_t*>(tile64 + tc::a_word_off<64>(r, c)) = w;
+}
+// the activation tile written by this warpgroup's threads becomes visible to its MMAs
+__device__ __forceinline__ void wg_publish(int bar_id) {
+  tc::fence_proxy_async_smem();
+  tc::named_sync(bar_id, 128);
+}
 
+struct Group {   // the 3-view group of this lane: the other two lanes
+  int l1, l2;
+  __device__ explicit Group(int lane) {
+    const int gb = 3 * (lane / 3);
+    l1 = (gb + (lane - gb + 1) % 3) & 31;
+    l2 = (gb + (lane - gb + 2) % 3) & 31;
+  }
+  __device__ float sum(float x) const { return x + __shfl_sync(FULL, x, l1) + __shfl_sync(FULL, x, l2); }
+  __device__ float min3(float x) const { return fminf(x, fminf(__shfl_sync(FULL, x, l1), __shfl_sync(FULL, x, l2))); }
+  __device__ float max3(float x) const { return fmaxf(x, fmaxf(__shfl_sync(FULL, x, l1), __shfl_sync(FULL, x, l2))); }
+};
+
+// =====================================================================================================================
+// geometry front: stages L0-L3 + view pooling.  Warpgroup tile = 64 rows: row warps 0/1 hold rows 0-31 / 32-63 with
+// column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
+// pooling columns, as tc_kmap's runs are laid out).  20 samples per tile.
+// =====================================================================================================================
+constexpr int GWG = 2;                        // warpgroups per CTA (front and tail kernels)
+constexpr int FSPT = 2 * SPW;                 // samples per front tile
+constexpr int D3S = 68;                       // row stride (floats) of the L3 accumulator rows staged for the pooling
+constexpr int POOL_W = 128;                   // pooled [mean 64 | var 64] fp32 per sample
+constexpr long long POOL_SLICE = 1ll << 22;   // samples per front/tail launch pair (bounds the pooled scratch to 2 GiB)
+__host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) { return 64u * (uint32_t)tc_k0p(n_kpt) * 2u; }
+static_assert(64 * D3S * 4 <= 64 * 192 * 2, "the L3 rows fit in the activation tile they replace");
+
+// one geometry stage of the warpgroup: A (64 rows at `a`) x resident W tile at `b` -> d (N = 128 or 64 fp32 per row)
+template <int N, int KCH>
+__device__ __forceinline__ void front_mma(float* d, const uint8_t* a, uint32_t b, int bar_id) {
+  wg_publish(bar_id);
+  tc::wg_fence();
+  tc::wg_mma<N, KCH>(d, tc::smem_u32(a), 1024u, b, (uint32_t)(N / 8) * 128u, 0u);
+  tc::wg_commit();
+  tc::wg_wait0();
+  tc::named_sync(bar_id, 128);   // every warp's MMAs are complete: the tile may be overwritten
+}
+// softplus epilogue of a 128-wide stage on the fragments: next layer's input words [0, 64); bias_tail: words 60..63 become
+// (1,0),0,0,0 (layer-3 input: bias column + K padding)
+__device__ __forceinline__ void front_epi_sp(const float* d, uint8_t* a, int wq, int lane, bool bias_tail) {
+#pragma unroll
+  for (int m = 0; m < 32; ++m) {
+    const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);
+    uint32_t w = sp_pair(__float_as_uint(d[2 * m]), __float_as_uint(d[2 * m + 1]));
+    if (bias_tail && m >= 30) w = (lane & 3) == 0 ? H2_ONE : 0u;
+    a_word(a, r, c, w);
+  }
+}
+
+template <int NK>
+__global__ void __launch_bounds__(GWG * 128, 1)
+geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ wblob, SampleSrc src, const int* __restrict__ list,
+                 const int* __restrict__ count_ptr, long long base, long long len, float* __restrict__ pool) {
+  extern __shared__ __align__(1024) uint8_t wsm[];
+  __shared__ uint64_t wbar;
+  __shared__ SceneS scs;
+  constexpr TcPlan plan = make_tc_plan(NK);
+  constexpr uint32_t WBYTES = plan.st[4].off;        // W_hi of stages 0..3
+  constexpr int NP = NK / 2, PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
+  const long long end = min((long long)*count_ptr, base + len);
+  if (end <= base) return;
+  const int ntiles = (int)((end - base + FSPT - 1) / FSPT);
+  const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31;
+  stage_scene(scs, *scp, NK, t, GWG * 128);
+  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
+  __syncthreads();
+  if (t == 0) load_weights(wsm, wblob, WBYTES, &wbar);
+  __syncthreads();
+  uint8_t* A = wsm + WBYTES + (size_t)wg * front_tile_bytes(NK);
+  float* D3 = reinterpret_cast<float*>(A);
+  const uint32_t W = tc::smem_u32(wsm);
+  const int bar_id = 1 + wg;
+  const int row = (wq & 1) * 32 + lane, h = wq >> 1;
+  const int g = lane / 3, v = lane - 3 * g;           // lanes 30, 31 replay views 0, 1 of the warp's last sample (unused)
+  const Group grp(lane);
+  for (int tile = blockIdx.x * GWG + wg; tile < ntiles; tile += gridDim.x * GWG) {
+    const long long si = base + (long long)tile * FSPT + (wq & 1) * SPW + min(g, SPW - 1);
+    const int id = list[min(si, end - 1)];
+    float p[3], dd[3];
+    fetch_sample(src, id, p, dd);
+    const Proj q = project_s(scs, v, p);
+    const float bw = boundary_weight_fast(q);
+    const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
+    // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap
+    {
+      float c[3];
+      const float* E = scs.E[v];
+      c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
+      c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
+      c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
+      const Taps t64 = make_taps(q.u, q.v, scs.f64.W, scs.f64.H);
+      if (h == 0) {
+        constexpr int N0 = 7 * PA + FA / 2;
+        uint32_t a[N0];
+#pragma unroll
+        for (int gq = 0; gq < FA / 4; ++gq) {
+          float f[4];
+          gather_f32<1>(scs.f64, v, t64, gq, f);
+          a[7 * PA + 2 * gq] = tc::pack_h2(f[0], f[1]);
+          a[7 * PA + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
+        }
+#pragma unroll
+        for (int j = 0; j < PA; ++j) {
+          float e0[7], e1[7];
+          encode_fast(scs, v, 2 * j, c, e0);
+          encode_fast(scs, v, 2 * j + 1, c, e1);
+#pragma unroll
+          for (int r = 0; r < 7; ++r) a[7 * j + r] = tc::pack_h2(e0[r], e1[r]);
+        }
+        a_put<64, N0>(A, row, 0, a);
+      } else {
+        constexpr int C1 = 7 * PA + FA / 2;           // first column of this thread's run
+        constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
+        constexpr int N1 = tc_k0p(NK) / 2 - C1;
+        uint32_t a[N1];
+#pragma unroll
+        for (int gq = 0; gq < (64 - FA) / 4; ++gq) {
+          float f[4];
+          gather_f32<1>(scs.f64, v, t64, FA / 4 + gq, f);
+          a[NE + 2 * gq] = tc::pack_h2(f[0], f[1]);
+          a[NE + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
+        }
+#pragma unroll
+        for (int j = PA; j < NP; ++j) {
+          float e0[7], e1[7];
+          encode_fast(scs, v, 2 * j, c, e0);
+          encode_fast(scs, v, 2 * j + 1, c, e1);
+#pragma unroll
+          for (int r = 0; r < 7; ++r) a[7 * (j - PA) + r] = tc::pack_h2(e0[r], e1[r]);
+        }
+        a[NE + NF] = H2_ONE;
+#pragma unroll
+        for (int i = NE + NF + 1; i < N1; ++i) a[i] = 0u;
+        static_assert(C1 % 4 == 0, "run starts on a 16-byte chunk");
+        a_put<64, N1>(A, row, C1, a);
+      }
+    }
+    // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720)
+    float d[64];
+    front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
+    front_epi_sp(d, A, wq, lane, false);
+    if (h == 0) {   // layer-1 input: bias chunk
+      const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+      a_put<64, 8>(A, row, 64, b);
+    }
+    front_mma<128, 9>(d, A, W + plan.st[1].off, bar_id);
+    front_epi_sp(d, A, wq, lane, false);
+    if (h == 1) {   // layer-2 input: feat8 | bias chunk
+      uint32_t b[8] = {0u, 0u, 0u, 0u, H2_ONE, 0u, 0u, 0u};
+      const Taps t8 = make_taps(q.u, q.v, scs.f8.W, scs.f8.H);
+      float g8[8];
+      gather_f32<2>(scs.f8, v, t8, 0, g8);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) b[i] = tc::pack_h2(g8[2 * i], g8[2 * i + 1]);
+      a_put<64, 8>(A, row, 64, b);
+    }
+    front_mma<128, 9>(d, A, W + plan.st[2].off, bar_id);
+    front_epi_sp(d, A, wq, lane, true);
+    front_mma<64, 8>(d, A, W + plan.st[3].off, bar_id);
+    // ---- L3 rows to shared memory (over the dead activation tile), then the view pooling: weighted mean || variance over
+    //      the 3 lanes of the group (src/utils.py:722-748); this thread owns 32 of the 64 feature columns
+#pragma unroll
+    for (int m = 0; m < 16; ++m) {
+      const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 8 * (m >> 1) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(D3 + r * D3S + c) = make_float2(d[2 * m], d[2 * m + 1]);
+    }
+    tc::named_sync(bar_id, 128);
+    {
+      const bool writer = lane < 3 * SPW && v == 0 && si < end;
+      float* out = pool + (si - base) * POOL_W + 32 * h;
+      const float* x = D3 + row * D3S + 32 * h;
+#pragma unroll
+      for (int c4 = 0; c4 < 8; ++c4) {
+        const float4 xv = *reinterpret_cast<const float4*>(x + 4 * c4);
+        const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+        float mn[4], vr[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          mn[i] = grp.sum(pw * xs[i]);
+          const float dl = xs[i] - mn[i];
+          vr[i] = grp.sum(pw * dl * dl);
+        }
+        if (writer) {
+          *reinterpret_cast<float4*>(out + 4 * c4) = make_float4(mn[0], mn[1], mn[2], mn[3]);
+          *reinterpret_cast<float4*>(out + 64 + 4 * c4) = make_float4(vr[0], vr[1], vr[2], vr[3]);
+        }
+      }
+    }
+    tc::named_sync(bar_id, 128);   // the L3 rows are read: the next tile's input may overwrite them
+  }
+}
+
+// =====================================================================================================================
+// geometry tail: P0|compress and P1 per sample (64 samples per warpgroup tile, two threads per row for the input build),
+// two-term weights and activations: D = A_hi W_hi [+ A_hi W_lo] [+ A_lo W_hi] (lo_mask bits 4/5: W_lo of stage 4/5,
+// bits 6/7: A_lo of stage 4/5).  Everything after the input build runs on the accumulator fragments.
+// =====================================================================================================================
+constexpr uint32_t T4H = 64 * 144 * 2, T4L = 64 * 128 * 2, T5H = 64 * 80 * 2, T5L = 64 * 64 * 2;   // activation tiles
+constexpr uint32_t TAIL_TILE_BYTES = T4H + T4L + T5H + T5L;
+
+template <int N, int KH, int KL>
+__device__ __forceinline__ void tail_mma(float* d, const uint8_t* ahi, const uint8_t* alo, uint32_t whi, uint32_t wlo, bool w_lo,
+                                         bool a_lo, int bar_id) {
+  constexpr uint32_t lbo = (uint32_t)(N / 8) * 128u;
+  wg_publish(bar_id);
+  tc::wg_fence();
+  tc::wg_mma<N, KH>(d, tc::smem_u32(ahi), 1024u, whi, lbo, 0u);
+  if (w_lo) tc::wg_mma<N, KH>(d, tc::smem_u32(ahi), 1024u, wlo, lbo, 1u);
+  if (a_lo) tc::wg_mma<N, KL>(d, tc::smem_u32(alo), 1024u, whi, lbo, 1u);
+  tc::wg_commit();
+  tc::wg_wait0();
+  tc::named_sync(bar_id, 128);
+}
+
+template <int NK>
+__global__ void __launch_bounds__(GWG * 128, 1)
+geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wblob, const uint8_t* __restrict__ wlo, int lo_mask,
+                const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
+                const float* __restrict__ pool, int query_mode, ShadeOut so, uint4* __restrict__ lat_out) {
+  extern __shared__ __align__(1024) uint8_t wsm[];
+  __shared__ uint64_t wbar;
+  __shared__ __align__(16) float wp2[132];                 // density head: w[0][64] | w[1][64] | b[2]
+  constexpr TcPlan plan = make_tc_plan(NK);
+  constexpr uint32_t HOFF = plan.st[4].off, WH = plan.st[GEO_NSTAGE].off - plan.st[4].off;   // W_hi of stages 4, 5
+  const long long end = min((long long)*count_ptr, base + len);
+  if (end <= base) return;
+  const int ntiles = (int)((end - base + 63) / 64);
+  const int t = threadIdx.x, wg = t >> 7, wt = t & 127, wq = wt >> 5, lane = t & 31;
+  for (int i = t; i < 130; i += GWG * 128) wp2[i] = i < 64 ? C.w_p2[0][i] : i < 128 ? C.w_p2[1][i - 64] : C.b_p2[i - 128];
+  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
+  __syncthreads();
+  if (t == 0) {   // [W_hi 4 | W_hi 5 | W_lo 4 | W_lo 5]
+    tc::mbar_expect_tx(&wbar, 2 * WH);
+    tc::bulk_g2s(wsm, wblob + HOFF, WH, &wbar);
+    tc::bulk_g2s(wsm + WH, wlo, WH, &wbar);
+    tc::mbar_wait(&wbar, 0, 0x31u);
+  }
+  __syncthreads();
+  uint8_t* A4h = wsm + 2 * WH + (size_t)wg * TAIL_TILE_BYTES;
+  uint8_t* A4l = A4h + T4H;
+  uint8_t* A5h = A4l + T4L;
+  uint8_t* A5l = A5h + T5H;
+  const uint32_t W4h = tc::smem_u32(wsm), W5h = W4h + (plan.st[5].off - HOFF), W4l = W4h + WH, W5l = W5h + WH;
+  const int bar_id = 1 + wg;
+  const int row = wt & 63, h = wt >> 6;
+  if (h == 0) {   // bias chunks of the two stages' inputs (never overwritten)
+    const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+    a_put<64, 8>(A4h, row, 64, b);
+    a_put<64, 8>(A5h, row, 32, b);
+  }
+  for (int tile = blockIdx.x * GWG + wg; tile < ntiles; tile += gridDim.x * GWG) {
+    const long long t0 = base + (long long)tile * 64;
+    {   // P0|compress input: [mean hi | var hi | bias chunk], [mean lo | var lo]
+      const long long si = min(t0 + row, end - 1);
+      const float* in = pool + (si - base) * POOL_W + 32 * h;
+      uint32_t mh[16], ml[16], vh[16], vl[16];
+#pragma unroll
+      for (int c4 = 0; c4 < 8; ++c4) {
+        const float4 m = __ldg(reinterpret_cast<const float4*>(in) + c4);
+        const float4 s = __ldg(reinterpret_cast<const float4*>(in + 64) + c4);
+        split_h2(m.x, m.y, mh[2 * c4], ml[2 * c4]);
+        split_h2(m.z, m.w, mh[2 * c4 + 1], ml[2 * c4 + 1]);
+        split_h2(s.x, s.y, vh[2 * c4], vl[2 * c4]);
+        split_h2(s.z, s.w, vh[2 * c4 + 1], vl[2 * c4 + 1]);
+      }
+      a_put<64, 16>(A4h, row, 16 * h, mh);
+      a_put<64, 16>(A4h, row, 32 + 16 * h, vh);
+      a_put<64, 16>(A4l, row, 16 * h, ml);
+      a_put<64, 16>(A4l, row, 32 + 16 * h, vl);
+    }
+    // ---- P0 (softplus, two fp16 terms out) | compress (linear, fp16 latent kept in registers until the density is known)
+    uint32_t lat[2][3];
+    {
+      float d[48];
+      tail_mma<96, 9, 8>(d, A4h, A4l, W4h, W4l, (lo_mask >> 4) & 1, (lo_mask >> 6) & 1, bar_id);
+#pragma unroll
+      for (int m = 0; m < 24; ++m) {
+        const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);
+        if (m < 16) {
+          uint32_t hi, lo;
+          split_h2(sp_fast(d[2 * m]), sp_fast(d[2 * m + 1]), hi, lo);
+          a_word(A5h, r, c, hi);
+          a_word(A5l, r, c, lo);
+        } else if (m < 22) {
+          lat[m & 1][(m >> 1) - 8] = tc::pack_h2(d[2 * m], d[2 * m + 1]);
+        }
+      }
+    }
+    // ---- P1 (softplus) then the 64->2 density head in fp32: partial dots over this lane's 16 columns, summed over the quad
+    float gs[2] = {0.0f, 0.0f}, rs[2] = {0.0f, 0.0f};
+    {
+      float d[32];
+      tail_mma<64, 5, 4>(d, A5h, A5l, W5h, W5l, (lo_mask >> 5) & 1, (lo_mask >> 7) & 1, bar_id);
+#pragma unroll
+      for (int m = 0; m < 16; ++m) {
+        const int c = 8 * (m >> 1) + 2 * (lane & 3);
+        const float h0 = sp_fast(d[2 * m]), h1 = sp_fast(d[2 * m + 1]);
+        gs[m & 1] = fmaf(wp2[c], h0, fmaf(wp2[c + 1], h1, gs[m & 1]));
+        rs[m & 1] = fmaf(wp2[64 + c], h0, fmaf(wp2[65 + c], h1, rs[m & 1]));
+      }
+    }
+    // ---- outputs (eval_func, src/model.py:978-997): alpha / sdf and, where a colour will be needed (density > 0: a sample with
+    //      alpha == 0 composites with weight exactly 0, skipping its colour is exact; every valid sample in query mode), the
+    //      compressed latent at the sample's own list index
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      float g0 = gs[k], rad = rs[k];
+      g0 += __shfl_xor_sync(FULL, g0, 1); g0 += __shfl_xor_sync(FULL, g0, 2);
+      rad += __shfl_xor_sync(FULL, rad, 1); rad += __shfl_xor_sync(FULL, rad, 2);
+      g0 += wp2[128];
+      rad += wp2[129];
+      const long long si = t0 + 16 * wq + (lane >> 2) + 8 * k;
+      if (si < end) {
+        if ((lane & 3) == 0) {
+          if (query_mode) {
+            float* o = so.out5 + 5ll * list[si];
+            o[0] = g0; o[1] = rad; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f;
+          } else {
+            so.ao[so.list_base + si] = make_float2(fmaxf(rad, 0.0f), g0);
+          }
+        }
+        if (query_mode != 0 || rad > 0.0f) {
+          uint32_t* lw = reinterpret_cast<uint32_t*>(lat_out + 3ll * si);
+#pragma unroll
+          for (int j = 0; j < 3; ++j) lw[4 * j + (lane & 3)] = lat[k][j];
+        }
+      }
+    }
+  }
+}
+
+// =====================================================================================================================
+// colour head.  Warpgroup tile = 128 rows (4 row warps x 10 samples x 3 views); each stage runs as two 64-row MMAs whose
+// accumulators are staged in shared memory (D) for the row threads, which do the cross-view work of the reference.
+// =====================================================================================================================
+constexpr int CWG = 2;                                   // warpgroups per CTA
+constexpr int CDS = 68;                                  // row stride (floats) of the staged accumulators
+constexpr uint32_t CA_BYTES = 128 * 112 * 2;             // activation tile (widest colour input: BASE0, K = 112)
+constexpr uint32_t CD_BYTES = 128 * CDS * 4;
+
+struct ColCtx {
+  uint8_t* A;
+  float* D;
+  uint32_t wbase;   // shared address of the colour stages' weights (plan offset of stage 6 at 0)
+  int bar_id, row, wq, lane;
+  Group grp;
+};
+
+template <int NK, int STAGE>
+__device__ __forceinline__ void col_mma(const ColCtx& c) {
+  constexpr TcPlan plan = make_tc_plan(NK);
+  constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
+  const uint32_t b = c.wbase + (plan.st[STAGE].off - plan.st[GEO_NSTAGE].off);
+  wg_publish(c.bar_id);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    float d[Np / 2];
+    tc::wg_fence();
+    tc::wg_mma<Np, Kp / 16>(d, tc::smem_u32(c.A) + 1024u * (uint32_t)half, 2048u, b, (uint32_t)(Np / 8) * 128u, 0u);
+    tc::wg_commit();
+    tc::wg_wait0();
+#pragma unroll
+    for (int m = 0; m < Np / 4; ++m) {
+      const int r = 64 * half + 16 * c.wq + (c.lane >> 2) + 8 * (m & 1), col = 8 * (m >> 1) + 2 * (c.lane & 3);
+      *reinterpret_cast<float2*>(c.D + r * CDS + col) = make_float2(d[2 * m], d[2 * m + 1]);
+    }
+  }
+  tc::named_sync(c.bar_id, 128);   // accumulators staged, every MMA has read the activation tile
+}
+template <int N>
+__device__ __forceinline__ void d_get(const ColCtx& c, int c0, float* x) {
+#pragma unroll
+  for (int i = 0; i < N; i += 4) {
+    const float4 f = *reinterpret_cast<const float4*>(c.D + c.row * CDS + c0 + i);
+    x[i] = f.x; x[i + 1] = f.y; x[i + 2] = f.z; x[i + 3] = f.w;
+  }
+}
+// staged accumulator columns [0, 32*NCH) -> act(acc + bias) as the next input's words [0, 16*NCH)
+template <int NCH, int ACT>  // ACT 1 = softplus100, 2 = ELU
+__device__ __forceinline__ void col_epi(const ColCtx& c, const float* __restrict__ bias) {
+#pragma unroll
+  for (int ch = 0; ch < NCH; ++ch) {
+    float x[32];
+    d_get<32>(c, 32 * ch, x);
+    uint32_t o[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      float x0 = x[2 * i] + bias[ch * 32 + 2 * i], x1 = x[2 * i + 1] + bias[ch * 32 + 2 * i + 1];
+      if (ACT == 1) { x0 = sp_fast(x0); x1 = sp_fast(x1); }
+      else { x0 = elu_fast(x0); x1 = elu_fast(x1); }
+      o[i] = tc::pack_h2(x0, x1);
+    }
+    a_put<128, 16>(c.A, c.row, 16 * ch, o);
+  }
+}
+
+// Colour pass for one tile of the second work list (entries: x = slot of the latent in the scratch buffer, y = sample id).
 template <int NK>
 __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, const SampleSrc& src,
                                            const int2* __restrict__ list2, const int* __restrict__ list1, int count, int tile,
-                                           RowCtx& cx, int roww, int lane,
-                                           const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
-  const uint32_t R0 = cx.R0, R1 = cx.R1;
+                                           const ColCtx& cx, const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
+  const int lane = cx.lane;
   const int g = lane / 3;
   const int v = lane - 3 * g;
-  const int si = tile * SPT + roww * SPW + min(g, SPW - 1);
+  const int si = tile * SPT + cx.wq * SPW + min(g, SPW - 1);
   const bool writer = (lane < 3 * SPW) && (v == 0) && (si < count);
   // entry: x = index into the first work list (where the latent sits and, + list_base, where the colour goes), y = sample id;
   // query mode shades every valid sample: the first list itself is the work list
@@ -831,35 +673,29 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
       for (int i = 0; i < 4; ++i) { acc0 = fmaf(C.w_re0[o][i], rd[i], acc0); acc1 = fmaf(C.w_re0[o + 1][i], rd[i], acc1); }
       a[o / 2] = tc::pack_h2(elu_fast(acc0), elu_fast(acc1));
     }
-    a[8] = 0x00003C00u;   // (1, 0): bias column
+    a[8] = H2_ONE;   // bias column
 #pragma unroll
     for (int i = 9; i < 16; ++i) a[i] = 0u;
-    tc::tmem_st16(R0, a);
-    signal_a(cx);
+    a_put<128, 16>(cx.A, cx.row, 0, a);
     col_mma<NK, 12>(cx);
-    wait_acc(cx);
-    uint32_t r[32], r2[8];
-    tc::tmem_ld32(R1, r);
-    tc::tmem_ld8(R1 + 32, r2);
-    tc::wait_ld();
+    float r[36];
+    d_get<36>(cx, 0, r);
 #pragma unroll
-    for (int o = 0; o < 32; ++o) f[o] += elu_fast(u2f(r[o]));
-#pragma unroll
-    for (int o = 32; o < 35; ++o) f[o] += elu_fast(u2f(r2[o - 32]));
+    for (int o = 0; o < 35; ++o) f[o] += elu_fast(r[o]);
   }
   float om;  // blending weight (src/model.py:1286-1289), mask == 1
   {
     float ex = ex2f(C.ani_abs * LOG2E * (rd[3] - 1.0f));
-    float e = ex - gmin(cx, ex);
-    om = e / (gsum(cx, e) + 1e-8f);
+    float e = ex - cx.grp.min3(ex);
+    om = e / (cx.grp.sum(e) + 1e-8f);
   }
   {  // BASE0 input [mean35 | var35 | f35 | 0-pad] (src/model.py:1291-1292)
     float mean[35], var[35];
 #pragma unroll
     for (int c = 0; c < 35; ++c) {
-      mean[c] = gsum(cx, om * f[c]);
+      mean[c] = cx.grp.sum(om * f[c]);
       float dl = f[c] - mean[c];
-      var[c] = gsum(cx, om * dl * dl);
+      var[c] = cx.grp.sum(om * dl * dl);
     }
     uint32_t a[56];
 #pragma unroll
@@ -871,62 +707,46 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
                  : e1 < 105 ? f[e1 >= 70 ? (e1 < 105 ? e1 - 70 : 0) : 0] : 0.0f;
       a[j] = tc::pack_h2(x0, x1);
     }
-    tc::tmem_st32(R0, a);
-    tc::tmem_st16(R0 + 32, a + 32);
-    tc::tmem_st8(R0 + 48, a + 48);
+    a_put<128, 56>(cx.A, cx.row, 0, a);
   }
-  signal_a(cx);
   col_mma<NK, 6>(cx);
   // ---- BASE0 -> BASE1
-  wait_acc(cx);
-  epi_inplace<2, 2>(R1, R1, C.b_base0);
-  signal_a(cx);
+  col_epi<2, 2>(cx, C.b_base0);
   col_mma<NK, 7>(cx);
-  wait_acc(cx);
   float x[32];
   {
-    uint32_t r[32];
-    tc::tmem_ld32(R0, r);
-    tc::wait_ld();
+    float r[32];
+    d_get<32>(cx, 0, r);
     uint32_t o[16];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) x[i] = elu_fast(u2f(r[i]) + C.b_base1[i]);
+    for (int i = 0; i < 32; ++i) x[i] = elu_fast(r[i] + C.b_base1[i]);
 #pragma unroll
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * om, x[2 * i + 1] * om);  // vis_layer1(x * weight)
-    tc::tmem_st16(R0, o);
+    a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  signal_a(cx);
   col_mma<NK, 8>(cx);
   // ---- VIS1A -> VIS1B (src/model.py:1294-1296)
-  wait_acc(cx);
-  epi_inplace<1, 2>(R1, R1, C.b_vis1a);
-  signal_a(cx);
+  col_epi<1, 2>(cx, C.b_vis1a);
   col_mma<NK, 9>(cx);
-  wait_acc(cx);
   {
-    uint32_t r[32], r2[16];
-    tc::tmem_ld32(R0, r);
-    tc::tmem_ld16(R0 + 32, r2);
-    tc::wait_ld();
-    float sg = sig_fast(elu_fast(u2f(r2[0]) + C.b_vis1b[32]));
+    float r[36];
+    d_get<36>(cx, 0, r);
+    float sg = sig_fast(elu_fast(r[32] + C.b_vis1b[32]));
     uint32_t o[16];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) x[i] += elu_fast(u2f(r[i]) + C.b_vis1b[i]);
+    for (int i = 0; i < 32; ++i) x[i] += elu_fast(r[i] + C.b_vis1b[i]);
 #pragma unroll
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * sg, x[2 * i + 1] * sg);  // x * sigmoid(vis) * mask
-    tc::tmem_st16(R0, o);
+    a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  signal_a(cx);
   col_mma<NK, 10>(cx);
   // ---- VIS2A (+ 32->1 sigmoid on CUDA cores) -> OUT0 input [x32 | vis | ray_diff4 | 0-pad] (src/model.py:1297-1300)
-  wait_acc(cx);
   {
-    uint32_t r[32];
-    tc::tmem_ld32(R1, r);
-    tc::wait_ld();
+    float r[32];
+    d_get<32>(cx, 0, r);
     float dot = C.b_vis2b;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) dot = fmaf(C.w_vis2b[i], elu_fast(u2f(r[i]) + C.b_vis2a[i]), dot);
+    for (int i = 0; i < 32; ++i) dot = fmaf(C.w_vis2b[i], elu_fast(r[i] + C.b_vis2a[i]), dot);
     float vis2 = sig_fast(dot);
     uint32_t o[24];
 #pragma unroll
@@ -936,21 +756,17 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     o[18] = tc::pack_h2(rd[3], 0.0f);
 #pragma unroll
     for (int i = 19; i < 24; ++i) o[i] = 0u;
-    tc::tmem_st16(R1, o);
-    tc::tmem_st8(R1 + 16, o + 16);
+    a_put<128, 24>(cx.A, cx.row, 0, o);
   }
-  signal_a(cx);
   col_mma<NK, 11>(cx);
   // ---- OUT0 -> 16->8->1 on CUDA cores -> softmax over the views -> blended colour (src/model.py:1300-1301)
-  wait_acc(cx);
   float logit;
   {
-    uint32_t r[16];
-    tc::tmem_ld16(R0, r);
-    tc::wait_ld();
+    float r[16];
+    d_get<16>(cx, 0, r);
     float h16[16];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) h16[i] = elu_fast(u2f(r[i]) + C.b_out0[i]);
+    for (int i = 0; i < 16; ++i) h16[i] = elu_fast(r[i] + C.b_out0[i]);
     logit = C.b_out2;
 #pragma unroll
     for (int o = 0; o < 8; ++o) {
@@ -961,9 +777,9 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     }
   }
   {
-    float e = ex2f((logit - gmax(cx, logit)) * LOG2E);
-    float inv = 1.0f / gsum(cx, e);
-    float r0 = gsum(cx, e * rgb[0]) * inv, r1 = gsum(cx, e * rgb[1]) * inv, r2 = gsum(cx, e * rgb[2]) * inv;
+    float e = ex2f((logit - cx.grp.max3(logit)) * LOG2E);
+    float inv = 1.0f / cx.grp.sum(e);
+    float r0 = cx.grp.sum(e * rgb[0]) * inv, r1 = cx.grp.sum(e * rgb[1]) * inv, r2 = cx.grp.sum(e * rgb[2]) * inv;
     if (writer) {
       float* o = query_mode ? so.out5 + 5ll * id + 2 : so.rgb + 3ll * (so.list_base + ent.x);
       o[0] = r0; o[1] = r1; o[2] = r2;
@@ -971,944 +787,112 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
   }
 }
 
-// Precision: the geometry/density weights (stages 0..5) are applied as W = W_hi + W_lo, two fp16 terms accumulated into
-// the same TMEM accumulator.  This removes the weight-rounding error, which is systematic along a ray and dominated the RGB
-// error of a plain fp16 pipeline (DESIGN.md "precision"); the tensor pipe has the headroom, the CUDA cores are the bottleneck.
-// Shared memory cannot hold two copies of the weights in one CTA, so the geometry kernel runs as CTA PAIRS (cta_group::2):
-// each CTA of a 2-CTA cluster keeps HALF of the output rows of every W_hi and W_lo tile resident, the pair's leader issues
-// M=256 MMAs that cover one tile of each CTA.
-constexpr int TC_NLO = 6;          // stages with a W_lo pass
-
-// which region holds the stage's A operand (bit = 1: R1); D goes to the other one.  Stages 1,3,4,7,9,11.
-constexpr uint32_t A_IN_R1 = 0xA9Au;
-
-// CTA-pair MMAs of one geometry stage, issued warp-converged (operands in uniform registers, one elected lane takes effect).
-// `wlo0`: low word of the shared-memory descriptor of this CTA's weight half-blob = [W_hi halves of stages 0..5 | W_lo halves]
-// (a stage's half tile sits at plan offset / 2; `lo_delta` = descriptor distance of the W_lo halves).  Per K chunk of 16 the
-// descriptor's start address advances by two core-matrix columns (2 * LBO).  Order: A_hi x W_hi, [A_hi x W_lo], [A_lo x W_hi].
-template <int NK, int STAGE>
-__device__ __forceinline__ void geo_issue(uint32_t slot_tm, uint32_t d_tm, uint32_t wlo0, uint32_t lo_delta, int lo_mask, uint32_t el) {
-  const bool two_term = (lo_mask >> STAGE) & 1, act_lo = STAGE >= 4 && ((lo_mask >> (STAGE + 2)) & 1);
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
-  constexpr uint32_t lbo = (uint32_t)(Np / 16) * 128u;   // half tile: Np/2 rows -> (Np/2)/8 core matrices per K column of 8
-  constexpr uint32_t idesc = tc::make_idesc_f16(256, Np);
-  constexpr uint32_t dhi = (128u >> 4) | (1u << 14);     // SBO = 128 bytes, descriptor version 1
-  constexpr uint32_t step = (2u * lbo) >> 4;
-  constexpr int NCH = Kp / 16;                                        // weight K chunks incl. the bias chunk
-  constexpr int NACT = STAGE == 4 ? 8 : STAGE == 5 ? 4 : NCH;         // chunks whose activations are contiguous from column 0
-  constexpr int BIASCOL = STAGE == 4 ? 128 : 64;                      // column of the separate bias chunk (stages 4, 5)
-  constexpr int LOCOL = STAGE == 4 ? 64 : 32;                         // first column of the A_lo half (stages 4, 5)
-  const uint32_t b0 = wlo0 + ((plan.st[STAGE].off / 2u) >> 4) + ((lbo >> 4) << 16);
-#pragma unroll
-  for (int j = 0; j < NCH; ++j)
-    tc::mma_ts2_el(d_tm, slot_tm + (uint32_t)(j < NACT ? 8 * j : BIASCOL), b0 + (uint32_t)j * step, dhi, idesc, j > 0 ? 1u : 0u, el);
-  if (two_term) {
-#pragma unroll
-    for (int j = 0; j < NCH; ++j)
-      tc::mma_ts2_el(d_tm, slot_tm + (uint32_t)(j < NACT ? 8 * j : BIASCOL), b0 + lo_delta + (uint32_t)j * step, dhi, idesc, 1u, el);
-  }
-  if (act_lo) {
-#pragma unroll
-    for (int j = 0; j < NACT; ++j)
-      tc::mma_ts2_el(d_tm, slot_tm + (uint32_t)(LOCOL + 8 * j), b0 + (uint32_t)j * step, dhi, idesc, 1u, el);
-  }
-}
-
-// MMAs of one colour stage on resident weights, issued warp-converged like geo_issue.  `wlo0`: descriptor low word of the
-// shared-memory base the colour stages' plan offsets are relative to (minus the first colour stage's offset).
-template <int NK, int STAGE>
-__device__ __forceinline__ void col_issue(uint32_t slot_tm, uint32_t wlo0, uint32_t el) {
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
-  constexpr uint32_t lbo = (uint32_t)(Np / 8) * 128u;
-  constexpr uint32_t idesc = tc::make_idesc_f16(128, Np);
-  constexpr uint32_t dhi = (128u >> 4) | (1u << 14);
-  constexpr uint32_t step = (2u * lbo) >> 4;
-  constexpr uint32_t a_r1 = (A_IN_R1 >> STAGE) & 1u;
-  const uint32_t a_tm = slot_tm + (a_r1 ? 64u : 0u), d_tm = slot_tm + (a_r1 ? 0u : 64u);
-  const uint32_t b0 = wlo0 + ((plan.st[STAGE].off - plan.st[GEO_NSTAGE].off) >> 4) + ((lbo >> 4) << 16);
-#pragma unroll
-  for (int j = 0; j < Kp / 16; ++j) tc::mma_ts_el(d_tm, a_tm + (uint32_t)j * 8u, b0 + (uint32_t)j * step, dhi, idesc, j > 0 ? 1u : 0u, el);
-}
-
-// issuer warp only: once the slot's four row warps have signalled this stage's input, issue its MMAs and commit
-template <int NK, int STAGE>
-__device__ __forceinline__ void col_mma(RowCtx& c) {
-  if (c.issuer) {
-    tc::mbar_wait(c.a_ready, c.pha, 0x50u + (uint32_t)STAGE);
-    c.pha ^= 1u;
-    tc::fence_after_sync();
-    col_issue<NK, STAGE>(c.slot_tm, c.wlo0, c.el);
-    tc::mma_commit_el(c.acc_ready, c.el);
-  }
-}
-
-__device__ __forceinline__ void stage_scene(SceneS& scs, const DevScene& g, int NK, int t, int nthreads) {
-  for (int i = t; i < 3 * 12; i += nthreads) { scs.P[i / 12][i % 12] = g.P[i / 12][i % 12]; scs.E[i / 12][i % 12] = g.E[i / 12][i % 12]; }
-  for (int i = t; i < 3 * 3; i += nthreads) scs.C[i / 3][i % 3] = g.C[i / 3][i % 3];
-  for (int i = t; i < 3 * NK; i += nthreads)
-    scs.kc[i / NK][i % NK] = make_float4(g.kc[i / NK][i % NK][0], g.kc[i / NK][i % NK][1], g.kc[i / NK][i % NK][2], 0.0f);
-  if (t == 0) {
-    scs.wm1 = g.wm1; scs.hm1 = g.hm1; scs.znear = g.znear; scs.inv_zrange = 1.0f / (g.zfar - g.znear);
-    scs.sp_scale = g.sp_scale; scs.inv2sig2 = g.inv2sig2; scs.inv_wm1 = 1.0f / g.wm1; scs.inv_hm1 = 1.0f / g.hm1;
-    scs.f64 = g.f64; scs.f8 = g.f8; scs.ftex = g.ftex; scs.img = g.img;
-  }
-}
-
-__device__ __forceinline__ void load_weights(uint8_t* dst, const uint8_t* src, uint32_t bytes, uint64_t* wbar) {
-  tc::mbar_expect_tx(wbar, bytes);
-  for (uint32_t off = 0; off < bytes; off += 32768u) {
-    uint32_t n = bytes - off < 32768u ? bytes - off : 32768u;
-    tc::bulk_g2s(dst + off, src + off, n, wbar);
-  }
-  tc::mbar_wait(wbar, 0, 0x30u);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// geometry + density kernel (CTA pairs; 16 row warps = 2 slots x 4 TMEM lane quarters x 2 column halves, + 1 control warp)
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int GEO_ROW_WARPS = 16;
-constexpr int GEO_THREADS = GEO_ROW_WARPS * 32;         // 512: no control warp (see GeoCtx::issuer)
-
 template <int NK>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEO_THREADS, 1)
-shade_geo_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wpair,
-                 int two_term, SampleSrc src, const int* __restrict__ list, const int* __restrict__ count_ptr,
-                 int query_mode, ShadeOut so, uint4* __restrict__ lat_out, int relaxed_arrive) {
-  extern __shared__ __align__(1024) uint8_t wsm[];
-  // barriers: [0] weights | per slot s: [1+2s] a_ready (one arrival per row warp of the pair = 16; only the leader's copy is
-  //           used), [2+2s] acc_ready (one multicast commit per stage, each CTA waits on its own copy)
-  __shared__ uint64_t bars[1 + 2 * NSLOT];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ SceneS scs;
-  __shared__ __align__(16) float wp2[132];                 // density head: w[0][64] | w[1][64] | b[2]
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr uint32_t WBYTES = plan.st[GEO_NSTAGE].off;   // per CTA: half of W_hi + half of W_lo of stages 0..5
-  constexpr bool PREF = geo_pref(NK);                    // gather staging buffer behind the weights
-  // warp index through a lane-0 broadcast: the compiler then keeps every warp-derived value (slot, lane quarter, column half,
-  // issuer flag, prefetch flags) in uniform registers and branches on them without convergence barriers (-8 % static code)
-  const int t = threadIdx.x, warp = __shfl_sync(FULL, t >> 5, 0), lane = t & 31;
-  const uint32_t rank = tc::cluster_ctarank();
-  const int cl = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-  const int count = *count_ptr;
-  const int ntiles = (count + SPT - 1) / SPT;
-  stage_scene(scs, *scp, NK, t, GEO_THREADS);
-  for (int i = t; i < 130; i += GEO_THREADS) wp2[i] = i < 64 ? C.w_p2[0][i] : i < 128 ? C.w_p2[1][i - 64] : C.b_p2[i - 128];
-
-  if (warp == 0) tc::tmem_alloc2(&tmem_base_s, 512);
-  if (t == 0) {
-    tc::mbar_init(&bars[0], 1);
-    for (int s = 0; s < NSLOT; ++s) { tc::mbar_init(&bars[1 + 2 * s], GEO_ROW_WARPS); tc::mbar_init(&bars[2 + 2 * s], 1); }
-    tc::fence_mbar_init();
-  }
-  __syncthreads();
-  if (t == 0) load_weights(wsm, wpair + (size_t)rank * WBYTES, WBYTES, &bars[0]);   // this CTA's half-blob
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();     // both CTAs: barriers initialised, TMEM allocated, weights resident
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-  // pair iteration i of slot s covers tiles 2*P and 2*P+1 with P = (i*ncl + cl)*NSLOT + s; this CTA takes tile 2*P + rank
-  {
-    const int slot = warp >> 3, q4 = warp & 3, h = (warp >> 2) & 1;   // TMEM lane quarter = warp id % 4
-    GeoCtx cx;
-    cx.tm = tbase + (uint32_t)slot * 256u + ((uint32_t)(q4 * 32) << 16);
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(cx.a_ready_cl) : "r"(tc::smem_u32(&bars[1 + 2 * slot])), "r"(0u));
-    cx.acc_ready = &bars[2 + 2 * slot];
-    cx.ph = 0;
-    cx.issuer = (rank == 0 && q4 == 0 && h == 0) ? 1 : 0;
-    cx.a_ready = &bars[1 + 2 * slot];
-    cx.pha = 0;
-    cx.slot_tm = tbase + (uint32_t)slot * 256u;
-    cx.wlo0 = (tc::smem_u32(wsm) >> 4) & 0x3FFFu;
-    cx.lod = (WBYTES / 2u) >> 4;
-    cx.el = tc::elect_one();
-    cx.lo_mask = two_term;
-    cx.relaxed = relaxed_arrive;
-    const int gb = 3 * (lane / 3);
-    cx.l1 = (gb + (lane - gb + 1) % 3) & 31;
-    cx.l2 = (gb + (lane - gb + 2) % 3) & 31;
-    const int bar_id = 1 + slot * 4 + q4;
-    uint32_t* fb = reinterpret_cast<uint32_t*>(wsm + WBYTES) + slot * (GEO_FW * 128) + 32 * q4 + lane;   // this row's staging column
-    GeoPre pre;
-    int parity = 0;
-    int P = cl * NSLOT + slot;
-    int nid = 0;
-    auto id_of_tile = [&](int tile) { return list[max(min(tile * SPT + q4 * SPW + min(lane / 3, SPW - 1), count - 1), 0)]; };
-    if (PREF && 2 * P < ntiles) {
-      geo_prefetch<NK>(scs, src, list, count, 2 * P + (int)rank, q4, h, lane, fb, 0, pre);
-      nid = id_of_tile(2 * (P + ncl * NSLOT) + (int)rank);
-    }
-    for (; 2 * P < ntiles; P += ncl * NSLOT) {
-      // a tile index past the end is a ghost tile: it replays the last sample, takes part in every barrier, writes nothing
-      const int Pn = P + ncl * NSLOT, Pn2 = Pn + ncl * NSLOT;
-      geo_tile<NK, PREF>(scs, wp2, src, list, count, 2 * P + (int)rank, 2 * Pn < ntiles ? 2 * Pn + (int)rank : -1,
-                         2 * Pn2 < ntiles ? 2 * Pn2 + (int)rank : -1, nid, fb, parity, pre, cx, q4, h, lane, bar_id, query_mode, so,
-                         lat_out);
-      parity ^= 1;
-    }
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();     // the peer's TMEM / barriers must outlive the leader's last MMA and commit
-  if (warp == 0) tc::tmem_dealloc2(tbase, 512);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// view-sequential geometry + density kernel (18 keypoints: the default geometry kernel there; engine 3 requests it explicitly)
-// ------------------------------------------------------------------------------------------------------------------
-// Same network, same resident two-term weights, same CTA pairs as shade_geo_kernel, other mapping of the work onto an SM:
-//   * a tile row is a SAMPLE (128 samples per CTA, 256 per pair), not a (sample, view) pair: the three views of a sample go
-//     through stages 0-3 one after the other in the same tensor-memory lane; the view pooling (reference
-//     src/utils.py:722-748) is thread-local: every view's 64-wide output is folded into running sums S1 = sum pw x,
-//     S2 = sum pw x^2 held in registers (mean = S1, var = S2 - S1^2 (2 - sum pw)); the pooled stages P0|compress and P1 run
-//     once per sample instead of once per (sample, view) row;
-//   * FOUR threads per row (16 row warps = 4 lane quarters x 4 column quarters): a stage's epilogue is 32 accumulator
-//     columns per thread and every row warp of the CTA works on the same stage; a 17th warp issues the MMAs;
-//   * TWO streams of 7 stages each in flight, each with its own activation / accumulator columns, interleaved in every row
-//     warp's program: stream B runs views 0 and 2 of the current tile except view 2's last stage, stream A the pooled stages of
-//     the PREVIOUS tile, view 1 of the current one and view 2's last stage (whose input the row warps write into A's columns);
-//     view 0 of the NEXT tile is built while that stage runs.  While the tensor core works on one stream's stage the row warps
-//     run the other's epilogue: 8 rounds per tile instead of 14 dependent stages;
-//   * 7 more warps only gather (below): the row warps never wait for global memory.
-// Tensor-memory columns (512): stream A: activations [0,136), accumulator [160,288) (its columns [96,128) double as the
-// exchange area of the four column quarters' partial density sums); stream B: activations [288,384), accumulator [384,512).
-constexpr int VS_A0 = 0, VS_D0 = 160, VS_A1 = 288, VS_D1 = 384;
-constexpr int VS_ROW_WARPS = 16;
-constexpr int VS_PROD_WARPS = 7;                              // gather producers (24 warps launched with 80 registers: row warps 72, the rest 96)
-constexpr int VS_THREADS = (VS_ROW_WARPS + 1 + VS_PROD_WARPS) * 32;
-// Gather staging: the producer warps blend the bilinear taps of every (row, view) pass into shared memory as packed fp16 pairs
-// (32 feat64 words + 4 feat8 words per row; feat64 word w of row r at vs_f64_word(w, r), feat8 word w at [w * 128 + r]); the row
-// warps' stage-0 / stage-2 builds only copy them.  feat64 buffers are released by the build that consumes them (2 buffers),
-// feat8 two rounds later (3 buffers).  They also stage every tile's sample positions and ids (loaded one tile ahead).
-constexpr int VS_F64_WORDS = 32 * 128, VS_F8_WORDS = 4 * 128;
-constexpr int VS_SMP_WORDS = 8 * 128;   // per tile and row: position (3), sample id, view weights (3), -; two tiles in flight
-constexpr int VS_STAGING_BYTES = (2 * VS_F64_WORDS + 3 * VS_F8_WORDS + 2 * VS_SMP_WORDS) * 4;
-
-struct VsCtx {
-  uint32_t tm;                 // tensor-memory base with this row's lane field
-  uint32_t a_ready_cl[2];      // cluster-mapped address of the LEADER CTA's a_ready barrier of stream 0 (A) / 1 (B)
-  uint64_t* acc_ready[2];      // this CTA's accumulator barriers
-  uint32_t ph[2];
-};
-__device__ __forceinline__ void vs_signal(const VsCtx& c, int s, int lane) {
-  tc::wait_st();
-  tc::fence_before_sync();
-  __syncwarp();
-  if (lane == 0) asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(c.a_ready_cl[s]) : "memory");
-}
-__device__ __forceinline__ void vs_wait(VsCtx& c, int s) {
-  tc::mbar_wait(c.acc_ready[s], c.ph[s], 0x70u + (uint32_t)s);
-  c.ph[s] ^= 1u;
-  tc::fence_after_sync();
-}
-// epilogue of a 128-wide softplus stage, this thread's 32 accumulator columns at d -> 16 packed columns at a
-__device__ __forceinline__ void vs_epi_sp(uint32_t d, uint32_t a, bool bias_tail) {
-  uint32_t r[32];
-  tc::tmem_ld32(d, r);
-  tc::wait_ld();
-  uint32_t o[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) o[i] = sp_pair(r[2 * i], r[2 * i + 1]);
-  if (bias_tail) { o[12] = H2_ONE; o[13] = 0u; o[14] = 0u; o[15] = 0u; }
-  tc::tmem_st16(a, o);
-}
-// Image coordinates of a sample for the gathers only: project_s with reciprocals instead of IEEE divisions (a few ulp in u, v --
-// the bilinear blend is continuous in them; validity and view weights use project_s).
-__device__ __forceinline__ void vs_project_uv(const SceneS& S, int v, const float p[3], float& u, float& w) {
-  const float* P = S.P[v];
-  const float hx = P[0] * p[0] + P[1] * p[1] + P[2] * p[2] + P[3];
-  const float hy = P[4] * p[0] + P[5] * p[1] + P[6] * p[2] + P[7];
-  const float hz = P[8] * p[0] + P[9] * p[1] + P[10] * p[2] + P[11];
-  const float iz = rcpf(hz);
-  u = 2.0f * (hx * iz) * S.inv_wm1 - 1.0f;
-  w = 2.0f * (hy * iz) * S.inv_hm1 - 1.0f;
-}
-// feat64 staging: word w (channels 2w, 2w + 1) of row r.  The producers write eight float4 groups of a row from eight adjacent
-// lanes; the XOR spreads them over the banks, and a row warp's 32 rows of one word stay on 32 banks.
-__device__ __forceinline__ int vs_f64_word(int w, int row) { return w * 128 + (row ^ (4 * ((w >> 1) & 7))); }
-struct VsSample { float p[3]; float pw[3]; int id, si, row; bool live; };
-#ifdef KPN_STAGE_TIMING
-// Instrumented build: cycle stamps of row warp 0 (row 0 of kpn_tim) and of the issuer warp (row 1) of block 0, per iteration
-// (tools/stage_times.py --vseq): row warp: [0] iteration start, [2n+1] n-th accumulator wait returned (the pooling build of
-// round 0 counts as a wait), [2n+2] the signal that follows it; issuer: [2g] operands of the g-th stage complete, [2g+1] committed.
-#define VT(idx) do { if (vt_on && lane == 0) kpn_tim[(size_t)it * TIM_WORDS + (idx)] = clock64(); } while (0)
-#define VI(idx) do { if (vi_on && el) kpn_tim[(size_t)(TIM_TILES + it) * TIM_WORDS + (idx)] = clock64(); } while (0)
-// producer warp 0: [0] iteration start, [1] samples staged, per view v: [2+4v] buffers free, [3+4v] last unit staged, [5+4v] arrived
-#define VP(idx) do { if (vp_on && lane == 0) kpn_tim[(size_t)(2 * TIM_TILES + it) * TIM_WORDS + (idx)] = clock64(); } while (0)
-#else
-#define VP(idx) do { } while (0)
-#define VT(idx) do { } while (0)
-#define VI(idx) do { } while (0)
-#endif
-
-// stage-0 input of (sample, view v): this thread's run of 24 columns (tc_kmap_vseq) at activation base `a`
-template <int NK>
-__device__ __forceinline__ void vs_build(const SceneS& sc, const VsSample& sm, int v, int cq, uint32_t a_tm,
-                                         const uint32_t* __restrict__ fbuf) {   // fbuf: the staged feat64 words of this pass
-  static_assert(NK == 18, "the column plan is the 18-keypoint one (4 runs of 24 columns)");
-  float c[3];
-  const float* E = sc.E[v];
-  c[0] = E[0] * sm.p[0] + E[1] * sm.p[1] + E[2] * sm.p[2] + E[3];
-  c[1] = E[4] * sm.p[0] + E[5] * sm.p[1] + E[6] * sm.p[2] + E[7];
-  c[2] = E[8] * sm.p[0] + E[9] * sm.p[1] + E[10] * sm.p[2] + E[11];
-  uint32_t a[24];
-  if (cq < 3) {
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      float e0[7], e1[7];
-      encode_fast(sc, v, 4 * cq + 2 * j, c, e0);
-      encode_fast(sc, v, 4 * cq + 2 * j + 1, c, e1);
-#pragma unroll
-      for (int r = 0; r < 7; ++r) a[7 * j + r] = tc::pack_h2(e0[r], e1[r]);
-    }
-#pragma unroll
-    for (int i = 0; i < 10; ++i) a[14 + i] = fbuf[vs_f64_word(10 * cq + i, sm.row)];   // float4 groups 5 cq .. 5 cq + 4
-  } else {
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      float e0[7], e1[7];
-      encode_fast(sc, v, 12 + 2 * j, c, e0);
-      encode_fast(sc, v, 13 + 2 * j, c, e1);
-#pragma unroll
-      for (int r = 0; r < 7; ++r) a[7 * j + r] = tc::pack_h2(e0[r], e1[r]);
-    }
-    a[21] = fbuf[vs_f64_word(30, sm.row)];   // float4 group 15
-    a[22] = fbuf[vs_f64_word(31, sm.row)];
-    a[23] = H2_ONE;
-  }
-  tc::tmem_st8(a_tm + 24u * (uint32_t)cq, a);
-  tc::tmem_st8(a_tm + 24u * (uint32_t)cq + 8u, a + 8);
-  tc::tmem_st8(a_tm + 24u * (uint32_t)cq + 16u, a + 16);
-}
-// [64,72) of the stage-2 input: feat8 | bias | 0 (thread 3)
-__device__ __forceinline__ void vs_feat8(const uint32_t* __restrict__ gcol, uint32_t a_tm) {   // gcol: this row's staged feat8 words
-  uint32_t b[8] = {0u, 0u, 0u, 0u, H2_ONE, 0u, 0u, 0u};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) b[i] = gcol[i * 128];
-  tc::tmem_st8(a_tm + 64, b);
-}
-// L3 accumulator (this thread's 16 of the 64 columns at d) folded into the pooling sums with the view's weight
-__device__ __forceinline__ void vs_accumulate(uint32_t d, float pw, float (&s1)[16], float (&s2)[16]) {
-  uint32_t x[16];
-  tc::tmem_ld16(d, x);
-  tc::wait_ld();
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const float xv = u2f(x[i]), t = pw * xv;
-    s1[i] += t;
-    s2[i] = fmaf(t, xv, s2[i]);
-  }
-}
-
-template <int NK>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(VS_THREADS, 1)   // 24 warps x 80 registers, redistributed by setmaxnreg
-shade_geo_vseq_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wpair,
-                      int two_term, SampleSrc src, const int* __restrict__ list, const int* __restrict__ count_ptr,
-                      int query_mode, ShadeOut so, uint4* __restrict__ lat_out, int fake_gather) {
-  extern __shared__ __align__(1024) uint8_t wsm[];
-  // barriers: [0] weights | [1], [2] a_ready of stream A, B (32 row-warp arrivals of the pair; only the leader's copies are used) |
-  //           [3], [4] acc_ready of stream A, B (one multicast commit per stage, each CTA waits on its own copy)
-  //           [5],[6] full / [7],[8] empty of the two feat64 staging buffers | [9..11] full / [12..14] empty of the three feat8 ones
-  //           | [15],[16] full / [17],[18] empty of the two per-tile sample buffers
-  __shared__ uint64_t bars[19];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ SceneS scs;
-  __shared__ __align__(16) float wp2[132];
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr uint32_t WBYTES = plan.st[GEO_NSTAGE].off;
-  const int t = threadIdx.x, warp = __shfl_sync(FULL, t >> 5, 0), lane = t & 31;
-  const uint32_t rank = tc::cluster_ctarank();
-  const int cl = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-  const int count = *count_ptr;
-  const int ntiles = (count + 127) / 128;
-  uint32_t* const stg64 = reinterpret_cast<uint32_t*>(wsm + WBYTES);          // [2][32][128]
-  uint32_t* const stg8 = stg64 + 2 * VS_F64_WORDS;                             // [3][4][128]
-  uint64_t* const fullF = &bars[5];
-  uint64_t* const emptyF = &bars[7];
-  uint64_t* const fullG = &bars[9];
-  uint64_t* const emptyG = &bars[12];
-  uint32_t* const stgS = stg8 + 3 * VS_F8_WORDS;                               // [2][8][128]
-  uint64_t* const fullS = &bars[15];
-  uint64_t* const emptyS = &bars[17];
-  // pair iterations of this cluster that have a real tile; one more iteration flushes the last tile's pooled stages
-  const int npair = (ntiles + 1) / 2;
-  const int nreal = npair > cl ? (npair - cl + ncl - 1) / ncl : 0;
-  stage_scene(scs, *scp, NK, t, VS_THREADS);
-  for (int i = t; i < 130; i += VS_THREADS) wp2[i] = i < 64 ? C.w_p2[0][i] : i < 128 ? C.w_p2[1][i - 64] : C.b_p2[i - 128];
-  if (warp == 0) tc::tmem_alloc2(&tmem_base_s, 512);
-  if (t == 0) {
-    tc::mbar_init(&bars[0], 1);
-    tc::mbar_init(&bars[1], 2 * VS_ROW_WARPS);
-    tc::mbar_init(&bars[2], 2 * VS_ROW_WARPS);
-    tc::mbar_init(&bars[3], 1);
-    tc::mbar_init(&bars[4], 1);
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&fullF[i], VS_PROD_WARPS); tc::mbar_init(&emptyF[i], VS_ROW_WARPS); }
-    for (int i = 0; i < 3; ++i) { tc::mbar_init(&fullG[i], VS_PROD_WARPS); tc::mbar_init(&emptyG[i], 4); }   // feat8: the 4 column-quarter-3 warps
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&fullS[i], VS_PROD_WARPS); tc::mbar_init(&emptyS[i], VS_ROW_WARPS); }
-    tc::fence_mbar_init();
-  }
-  __syncthreads();
-  if (t == 0) load_weights(wsm, wpair + (size_t)rank * WBYTES, WBYTES, &bars[0]);
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::cluster_sync_all();
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-#ifdef KPN_STAGE_TIMING
-  const long long blk_t0 = clock64();
-  const int tim_blk = fake_gather >> 8;
-  fake_gather &= 0xff;
-#endif
-  // registers: the row warps hand 8 per thread to the issuer / producer warps, whose gathers keep 16 tap loads (64 registers) in
-  // flight per thread -- global-memory latency times loads in flight is what bounds the producers
-  static_assert(VS_ROW_WARPS % 4 == 0 && (VS_THREADS / 32) % 4 == 0 &&
-                VS_ROW_WARPS * 72 + (VS_THREADS / 32 - VS_ROW_WARPS) * 96 <= (VS_THREADS / 32) * 80,
-                "whole warpgroups change their budget, and what the producers take the row warps must have released (else the "
-                "allocation spins forever)");
-  if (warp < VS_ROW_WARPS) asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-  else asm volatile("setmaxnreg.inc.sync.aligned.u32 96;");
-  if (warp == VS_ROW_WARPS) {
-    // ---- MMA issuer (leader CTA): the stages in the order the row warps signal them, two streams interleaved
-    if (rank == 0 && nreal > 0) {
-      const uint32_t wlo0 = (tc::smem_u32(wsm) >> 4) & 0x3FFFu, lod = (WBYTES / 2u) >> 4, el = tc::elect_one();
-      const uint32_t a_tm[2] = {tbase + (uint32_t)VS_A0, tbase + (uint32_t)VS_A1}, d_tm[2] = {tbase + (uint32_t)VS_D0, tbase + (uint32_t)VS_D1};
-      uint32_t pha[2] = {0u, 0u};
-      int it = 0, gi = 0;
-      auto go = [&](auto stage_c, int s) {
-        constexpr int STAGE = decltype(stage_c)::value;
-#ifdef KPN_STAGE_TIMING
-        const bool vi_on = (int)blockIdx.x == tim_blk && it < TIM_TILES;
-#endif
-        tc::mbar_wait(&bars[1 + s], pha[s], 0x60u + 8u * (uint32_t)s + (uint32_t)STAGE);
-        pha[s] ^= 1u;
-        tc::fence_after_sync();
-        VI(2 * gi);
-        geo_issue<NK, STAGE>(a_tm[s], d_tm[s], wlo0, lod, two_term, el);
-        tc::mma_commit2_el(&bars[3 + s], el);
-        VI(2 * gi + 1);
-        ++gi;
-      };
-      using std::integral_constant;
-      gi = 15;
-      go(integral_constant<int, 0>{}, 1);   // view 0 of the first tile
-      for (it = 0; it <= nreal; ++it) {
-        gi = 0;
-        go(integral_constant<int, 4>{}, 0);
-        go(integral_constant<int, 1>{}, 1); go(integral_constant<int, 5>{}, 0);
-        go(integral_constant<int, 2>{}, 1); go(integral_constant<int, 0>{}, 0);
-        go(integral_constant<int, 3>{}, 1); go(integral_constant<int, 1>{}, 0);
-        go(integral_constant<int, 0>{}, 1); go(integral_constant<int, 2>{}, 0);
-        go(integral_constant<int, 1>{}, 1); go(integral_constant<int, 3>{}, 0);
-        go(integral_constant<int, 2>{}, 1); go(integral_constant<int, 3>{}, 0);   // view 2's last stage runs on stream A's columns
-        if (it < nreal) go(integral_constant<int, 0>{}, 1);                          // view 0 of the next tile
-      }
-    }
-  } else if (warp > VS_ROW_WARPS) {
-    // ---- gather producers.  A pass = one view of one tile: 128 rows x (16 feat64 + 2 feat8) float4 groups, bilinear taps blended
-    //      in fp32 (reference src/utils.py:74-89), packed to fp16 pairs, staged for the row warps' builds.  Work unit = 4 rows
-    //      (warp u % 7 takes unit u of 32): lane l works on row 4u + l / 8 and feat64 groups l % 8 and 8 + l % 8, so that the eight
-    //      lanes of a row read one 128-byte line per tap and load (lanes l % 8 < 2 also blend the row's two feat8 groups).
-    if (nreal > 0) {
-      const int pw = warp - VS_ROW_WARPS - 1, pt = pw * 32 + lane;
-      const int l8 = lane & 7, lr = lane >> 3;
-      uint32_t phF[2] = {0u, 0u}, phG[3] = {0u, 0u, 0u}, phS[2] = {0u, 0u};
-      int k = 0;
-      // Samples of a tile (threads 0..127: one row each): id, then position (fetch_sample's arithmetic with 32-bit indices), both
-      // loaded one tile ahead -- the id under the view-0 gathers of the tile before, the position under its view-1 gathers -- and
-      // staged in shared memory for the row warps AND for the other producer threads
-      const int srow = min(pt, 127);
-      auto load_id = [&](int itn) {
-        const int tile = 2 * (cl + itn * ncl) + (int)rank;
-        return list[max(min(tile * 128 + srow, count - 1), 0)];
-      };
-      auto load_pos = [&](int id, float (&pos)[3]) {
-        if (src.mode == 0) {
-          const int r = (int)((unsigned)id / (unsigned)src.S);
-          const float z = src.z ? src.z[id] : coarse_depth(src.ray_nf[2 * r], src.ray_nf[2 * r + 1], id - r * src.S, src.S);
-          pos[0] = src.o[0] + src.ray_d[3 * r + 0] * z;   // eval_pts = cam_pos + cam_rays * z  (reference src/model.py:1057)
-          pos[1] = src.o[1] + src.ray_d[3 * r + 1] * z;
-          pos[2] = src.o[2] + src.ray_d[3 * r + 2] * z;
-        } else {
-          pos[0] = src.pts[3ll * id + 0]; pos[1] = src.pts[3ll * id + 1]; pos[2] = src.pts[3ll * id + 2];
-        }
-      };
-      int idc = load_id(0), idn = idc;
-      float pc[3], pn[3];
-      load_pos(idc, pc);
-      pn[0] = pc[0]; pn[1] = pc[1]; pn[2] = pc[2];
-      const float4* const b64 = (const float4*)scs.f64.ptr;
-      const float4* const b8 = (const float4*)scs.f8.ptr;
-      const int hw64 = scs.f64.H * scs.f64.W, hw8 = scs.f8.H * scs.f8.W;
-      for (int it = 0; it <= nreal; ++it) {
-#ifdef KPN_STAGE_TIMING
-        const bool vp_on = (int)blockIdx.x == tim_blk && warp == VS_ROW_WARPS + 1 && it < TIM_TILES;
-#endif
-        VP(0);
-        const int sb = it & 1;
-        if (it >= 2) { tc::mbar_wait(&emptyS[sb], phS[sb], 0x88u + (uint32_t)sb); phS[sb] ^= 1u; }
-        uint32_t* const smp = stgS + sb * VS_SMP_WORDS;
-        if (pt < 128) {
-          smp[pt] = __float_as_uint(pc[0]); smp[128 + pt] = __float_as_uint(pc[1]); smp[256 + pt] = __float_as_uint(pc[2]);
-          smp[384 + pt] = (uint32_t)idc;
-          float pwv[3], sum = 0.0f;   // view weights (reference src/model.py:750-759; mask == 1 for shaded samples)
-#pragma unroll
-          for (int vv = 0; vv < 3; ++vv) { const Proj q = project_s(scs, vv, pc); pwv[vv] = boundary_weight_fast(q); sum += pwv[vv]; }
-          const float inv = 1.0f / (sum + 1e-6f);
-#pragma unroll
-          for (int vv = 0; vv < 3; ++vv) smp[(4 + vv) * 128 + pt] = __float_as_uint(pwv[vv] * inv);
-        }
-        tc::named_sync(5, VS_PROD_WARPS * 32);   // every producer reads the positions below
-        if (lane == 0) tc::mbar_arrive(&fullS[sb]);
-        VP(1);
-        for (int v = 0; v < 3; ++v, ++k) {
-          const int fb = k & 1, gb = k % 3;
-          if (k >= 2) { tc::mbar_wait(&emptyF[fb], phF[fb], 0x80u + (uint32_t)fb); phF[fb] ^= 1u; }
-          if (k >= 3) { tc::mbar_wait(&emptyG[gb], phG[gb], 0x84u + (uint32_t)gb); phG[gb] ^= 1u; }
-          VP(2 + 4 * v);
-          if (it < nreal) {
-            if (v == 0) idn = load_id(it + 1);
-            if (v == 1) load_pos(idn, pn);
-          }
-          uint32_t* const f64b = stg64 + fb * VS_F64_WORDS;
-          uint32_t* const f8b = stg8 + gb * VS_F8_WORDS;
-          // three rounds of loads per pass and warp: feat64 units (pw, pw + 7), (pw + 14, pw + 21) with 16 tap loads in flight
-          // per thread, then unit pw + 28 (warps 0..3) together with the feat8 groups of 16 rows (lane l: row 16 pw + l / 2,
-          // group l % 2; warp 4 also takes the eighth such block)
-          auto taps_of = [&](int row, int W, int H) {
-            const float p[3] = {u2f(smp[row]), u2f(smp[128 + row]), u2f(smp[256 + row])};
-            float qu, qv;
-            vs_project_uv(scs, v, p, qu, qv);
-            return make_taps(qu, qv, W, H);
-          };
-          auto load64 = [&](const Taps& t, float4 (&a)[4], float4 (&c)[4]) {
-            const float4* const q = b64 + (v * hw64) * 16 + l8;
-            a[0] = __ldg(q + t.o00 * 16); a[1] = __ldg(q + t.o01 * 16); a[2] = __ldg(q + t.o10 * 16); a[3] = __ldg(q + t.o11 * 16);
-            c[0] = __ldg(q + t.o00 * 16 + 8); c[1] = __ldg(q + t.o01 * 16 + 8);
-            c[2] = __ldg(q + t.o10 * 16 + 8); c[3] = __ldg(q + t.o11 * 16 + 8);
-          };
-          auto blend2 = [&](const Taps& t, const float4 (&a)[4], uint32_t& w0, uint32_t& w1) {
-            w0 = tc::pack_h2(a[0].x * t.w00 + a[1].x * t.w01 + a[2].x * t.w10 + a[3].x * t.w11,
-                             a[0].y * t.w00 + a[1].y * t.w01 + a[2].y * t.w10 + a[3].y * t.w11);
-            w1 = tc::pack_h2(a[0].z * t.w00 + a[1].z * t.w01 + a[2].z * t.w10 + a[3].z * t.w11,
-                             a[0].w * t.w00 + a[1].w * t.w01 + a[2].w * t.w10 + a[3].w * t.w11);
-          };
-          auto store64 = [&](int row, const Taps& t, const float4 (&a)[4], const float4 (&c)[4]) {
-            uint32_t* const d = f64b + (2 * l8) * 128 + (row ^ (4 * l8));   // words 2g, 2g + 1 for g = l8, 8 + l8: see vs_f64_word
-            uint32_t w0, w1;
-            blend2(t, a, w0, w1);
-            d[0] = w0; d[128] = w1;
-            blend2(t, c, w0, w1);
-            d[16 * 128] = w0; d[17 * 128] = w1;
-          };
-          if (!fake_gather) {
-#pragma unroll
-            for (int rd = 0; rd < 2; ++rd) {
-              const int ra = 4 * (pw + 14 * rd) + lr, rb = ra + 28;
-              const Taps ta = taps_of(ra, scs.f64.W, scs.f64.H), tb = taps_of(rb, scs.f64.W, scs.f64.H);
-              float4 a[4], c[4], e[4], f[4];
-              load64(ta, a, c);
-              load64(tb, e, f);
-              store64(ra, ta, a, c);
-              store64(rb, tb, e, f);
-            }
-            {
-              const int r8 = 16 * pw + (lane >> 1), r8b = 112 + (lane >> 1), g8 = lane & 1;
-              const Taps t8 = taps_of(r8, scs.f8.W, scs.f8.H);
-              const float4* const q8 = b8 + (v * hw8) * 2 + g8;
-              float4 e[4] = {__ldg(q8 + t8.o00 * 2), __ldg(q8 + t8.o01 * 2), __ldg(q8 + t8.o10 * 2), __ldg(q8 + t8.o11 * 2)};
-              uint32_t w0, w1;
-              if (pw < 4) {
-                const int rc = 4 * (pw + 28) + lr;
-                const Taps tc64 = taps_of(rc, scs.f64.W, scs.f64.H);
-                float4 a[4], c[4];
-                load64(tc64, a, c);
-                store64(rc, tc64, a, c);
-              } else if (pw == 4) {
-                const Taps t8b = taps_of(r8b, scs.f8.W, scs.f8.H);
-                const float4 h[4] = {__ldg(q8 + t8b.o00 * 2), __ldg(q8 + t8b.o01 * 2), __ldg(q8 + t8b.o10 * 2), __ldg(q8 + t8b.o11 * 2)};
-                blend2(t8b, h, w0, w1);
-                f8b[(2 * g8) * 128 + r8b] = w0; f8b[(2 * g8 + 1) * 128 + r8b] = w1;
-              }
-              blend2(t8, e, w0, w1);
-              f8b[(2 * g8) * 128 + r8] = w0; f8b[(2 * g8 + 1) * 128 + r8] = w1;
-            }
-          }
-          VP(3 + 4 * v);
-          __syncwarp();
-          if (lane == 0) { tc::mbar_arrive(&fullF[fb]); tc::mbar_arrive(&fullG[gb]); }   // release: the warp's staged words are visible
-          VP(5 + 4 * v);
-        }
-        idc = idn; pc[0] = pn[0]; pc[1] = pn[1]; pc[2] = pn[2];
-      }
-    }
-  } else if (nreal > 0) {
-    const int q4 = warp & 3, cq = warp >> 2;   // TMEM lane quarter = warp id % 4; column quarter
-    VsCtx cx;
-    cx.tm = tbase + ((uint32_t)(q4 * 32) << 16);
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(cx.a_ready_cl[0]) : "r"(tc::smem_u32(&bars[1])), "r"(0u));
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(cx.a_ready_cl[1]) : "r"(tc::smem_u32(&bars[2])), "r"(0u));
-    cx.acc_ready[0] = &bars[3]; cx.acc_ready[1] = &bars[4];
-    cx.ph[0] = 0; cx.ph[1] = 0;
-    const uint32_t A0 = cx.tm + (uint32_t)VS_A0, D0 = cx.tm + (uint32_t)VS_D0, A1 = cx.tm + (uint32_t)VS_A1, D1 = cx.tm + (uint32_t)VS_D1;
-    const uint32_t c16 = 16u * (uint32_t)cq, c32 = 32u * (uint32_t)cq, c8 = 8u * (uint32_t)cq;
-    const uint32_t bias8[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-    float s1[16], s2[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) { s1[i] = 0.0f; s2[i] = 0.0f; }
-    VsSample cur;
-    cur.live = false; cur.id = 0; cur.si = 0; cur.pw[0] = cur.pw[1] = cur.pw[2] = 0.0f; cur.p[0] = cur.p[1] = cur.p[2] = 0.0f;
-    int prev_id = 0, prev_si = 0;
-    bool prev_live = false;
-    float prev_pw2 = 0.0f, prev_s0 = 0.0f;
-    uint32_t fphF[2] = {0u, 0u}, fphG[3] = {0u, 0u, 0u}, fphS[2] = {0u, 0u};   // parities of the staging buffers' "full" barriers
-    const int row = 32 * q4 + lane;
-    // the staged feat64 words of pass k (view k % 3 of iteration k / 3): wait until the producers have filled the buffer
-    auto feat64_of = [&](int k) -> const uint32_t* {
-      const int fb = k & 1;
-      tc::mbar_wait(&fullF[fb], fphF[fb], 0x90u + (uint32_t)fb);
-      fphF[fb] ^= 1u;
-      return stg64 + fb * VS_F64_WORDS;
-    };
-    auto feat64_done = [&](int k) {   // after the build has copied them: hand the buffer back
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&emptyF[k & 1]);
-    };
-    auto feat8_stage = [&](int k, uint32_t a_tm) {   // column-quarter-3 warps only
-      const int gb = k % 3;
-      tc::mbar_wait(&fullG[gb], fphG[gb], 0x94u + (uint32_t)gb);
-      fphG[gb] ^= 1u;
-      vs_feat8(stg8 + gb * VS_F8_WORDS + row, a_tm);
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&emptyG[gb]);
-    };
-    // sample of this row in iteration `itn` (position and id staged by the producers; a tile index past the end is a ghost: every
-    // barrier, no output) and its view-0 input -> stream B
-    auto start_tile = [&](int itn) {
-      const int tile = 2 * (cl + itn * ncl) + (int)rank;
-      const int sb = itn & 1;
-      tc::mbar_wait(&fullS[sb], fphS[sb], 0x98u + (uint32_t)sb);
-      fphS[sb] ^= 1u;
-      const uint32_t* sp = stgS + sb * VS_SMP_WORDS + row;
-      cur.si = tile * 128 + row;
-      cur.row = row;
-      cur.live = cur.si < count;
-      cur.p[0] = u2f(sp[0]); cur.p[1] = u2f(sp[128]); cur.p[2] = u2f(sp[256]);
-      cur.id = (int)sp[384];
-      cur.pw[0] = u2f(sp[512]); cur.pw[1] = u2f(sp[640]); cur.pw[2] = u2f(sp[768]);
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&emptyS[sb]);
-      vs_build<NK>(scs, cur, 0, cq, A1, feat64_of(3 * itn));
-      feat64_done(3 * itn);
-      vs_signal(cx, 1, lane);
-    };
-    start_tile(0);
-    for (int it = 0; it <= nreal; ++it) {
-#ifdef KPN_STAGE_TIMING
-      const bool vt_on = (int)blockIdx.x == tim_blk && warp == 0 && it < TIM_TILES;
-#endif
-      VT(0);
-      const int k0 = 3 * it;
-      // ================= round 0
-      // A: view 2 of the previous tile (its last stage ran on stream A's columns) -> pooling sums
-      if (it > 0) {
-        vs_wait(cx, 0);   VT(1);
-        vs_accumulate(D0 + c16, prev_pw2, s1, s2);
-      }
-      // A: pooling of the previous tile: mean = S1, var = S2 - S1^2 (2 - sum pw) (== sum pw (x - mean)^2), two fp16 terms each
-      {
-        uint32_t mh[8], vh[8], ml[8], vl[8];
-        const float k = 2.0f - prev_s0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float m0 = s1[2 * i], m1 = s1[2 * i + 1];
-          const float v0 = fmaf(-k * m0, m0, s2[2 * i]), v1 = fmaf(-k * m1, m1, s2[2 * i + 1]);
-          split_h2(m0, m1, mh[i], ml[i]);
-          split_h2(v0, v1, vh[i], vl[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < 16; ++i) { s1[i] = 0.0f; s2[i] = 0.0f; }
-        tc::tmem_st8(A0 + c8, mh);
-        tc::tmem_st8(A0 + 32u + c8, vh);
-        tc::tmem_st8(A0 + 64u + c8, ml);
-        tc::tmem_st8(A0 + 96u + c8, vl);
-        if (cq == 0) tc::tmem_st8(A0 + 128, bias8);
-      }
-      vs_signal(cx, 0, lane);   VT(2);
-      // ================= round 1
-      vs_wait(cx, 1);   VT(3);
-      vs_epi_sp(D1 + c32, A1 + c16, false);
-      if (cq == 0) tc::tmem_st8(A1 + 64, bias8);
-      vs_signal(cx, 1, lane);   VT(4);
-      // A: P0 (softplus, two fp16 terms out) | compress (linear; threads 0-2 keep 8 of the 24 latent values each)
-      uint32_t latq[4] = {0u, 0u, 0u, 0u};
-      vs_wait(cx, 0);   VT(5);
-      {
-        uint32_t r[16];
-        tc::tmem_ld16(D0 + c16, r);
-        if (cq < 3) {
-          uint32_t rc[8];
-          tc::tmem_ld8(D0 + 64u + c8, rc);
-          tc::wait_ld();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) latq[i] = tc::pack_h2(u2f(rc[2 * i]), u2f(rc[2 * i + 1]));
-        } else {
-          tc::wait_ld();
-        }
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) split_h2(sp_fast(u2f(r[2 * i])), sp_fast(u2f(r[2 * i + 1])), hi[i], lo[i]);
-        tc::tmem_st8(A0 + c8, hi);
-        tc::tmem_st8(A0 + 32u + c8, lo);
-        if (cq == 0) tc::tmem_st8(A0 + 64, bias8);
-      }
-      vs_signal(cx, 0, lane);   VT(6);
-      // ================= round 2
-      vs_wait(cx, 1);   VT(7);
-      vs_epi_sp(D1 + c32, A1 + c16, false);
-      if (cq == 3) feat8_stage(k0, A1);
-      vs_signal(cx, 1, lane);   VT(8);
-      // A: P1 (softplus) + the 64->2 density head in fp32 (partial dot over this thread's 16 columns; the four quarters meet
-      //    through 8 words each of the row's tensor-memory lane) + the previous tile's outputs; then view 1 of this tile
-      vs_wait(cx, 0);   VT(9);
-      {
-        float g0 = 0.0f, rad = 0.0f;
-        uint32_t r[16];
-        tc::tmem_ld16(D0 + c16, r);
-        tc::wait_ld();
-        const float* w0 = wp2 + 16 * cq;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float hh = sp_fast(u2f(r[i]));
-          g0 = fmaf(w0[i], hh, g0);
-          rad = fmaf(w0[64 + i], hh, rad);
-        }
-        const uint32_t xw[8] = {__float_as_uint(g0), __float_as_uint(rad), 0u, 0u, 0u, 0u, 0u, 0u};
-        tc::tmem_st8(D0 + 96u + c8, xw);
-        tc::wait_st();
-        tc::fence_before_sync();
-        tc::named_sync(1 + q4, 128);   // the four row warps of this lane quarter
-        tc::fence_after_sync();
-        uint32_t xr[32];
-        tc::tmem_ld32(D0 + 96u, xr);
-        tc::wait_ld();
-        g0 = (u2f(xr[0]) + u2f(xr[8])) + (u2f(xr[16]) + u2f(xr[24])) + wp2[128];
-        rad = (u2f(xr[1]) + u2f(xr[9])) + (u2f(xr[17]) + u2f(xr[25])) + wp2[129];
-        // outputs (as shade_geo_kernel): alpha / sdf record, latent where a colour will be needed
-        if (prev_live) {
-          if (cq == 0) {
-            if (query_mode) {
-              float* o = so.out5 + 5ll * prev_id;
-              o[0] = g0; o[1] = rad; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f;
-            } else {
-              so.ao[so.list_base + prev_si] = make_float2(fmaxf(rad, 0.0f), g0);
-            }
-          }
-          if (cq < 3 && (query_mode != 0 || rad > 0.0f)) lat_out[3ll * prev_si + cq] = make_uint4(latq[0], latq[1], latq[2], latq[3]);
-        }
-      }
-      vs_build<NK>(scs, cur, 1, cq, A0, feat64_of(k0 + 1));
-      feat64_done(k0 + 1);
-      vs_signal(cx, 0, lane);   VT(10);
-      // ================= round 3
-      vs_wait(cx, 1);   VT(11);
-      vs_epi_sp(D1 + c32, A1 + c16, cq == 3);   // layer-3 input: [0,60) act | 60 bias | 0
-      vs_signal(cx, 1, lane);   VT(12);
-      vs_wait(cx, 0);   VT(13);
-      vs_epi_sp(D0 + c32, A0 + c16, false);
-      if (cq == 0) tc::tmem_st8(A0 + 64, bias8);
-      vs_signal(cx, 0, lane);   VT(14);
-      // ================= round 4
-      vs_wait(cx, 1);   VT(15);
-      vs_accumulate(D1 + c16, cur.pw[0], s1, s2);
-      vs_build<NK>(scs, cur, 2, cq, A1, feat64_of(k0 + 2));
-      feat64_done(k0 + 2);
-      vs_signal(cx, 1, lane);   VT(16);
-      vs_wait(cx, 0);   VT(17);
-      vs_epi_sp(D0 + c32, A0 + c16, false);
-      if (cq == 3) feat8_stage(k0 + 1, A0);
-      vs_signal(cx, 0, lane);   VT(18);
-      // ================= round 5
-      vs_wait(cx, 1);   VT(19);
-      vs_epi_sp(D1 + c32, A1 + c16, false);
-      if (cq == 0) tc::tmem_st8(A1 + 64, bias8);
-      vs_signal(cx, 1, lane);   VT(20);
-      vs_wait(cx, 0);   VT(21);
-      vs_epi_sp(D0 + c32, A0 + c16, cq == 3);
-      vs_signal(cx, 0, lane);   VT(22);
-      // ================= round 6
-      vs_wait(cx, 1);   VT(23);
-      vs_epi_sp(D1 + c32, A1 + c16, false);
-      if (cq == 3) feat8_stage(k0 + 2, A1);
-      vs_signal(cx, 1, lane);   VT(24);
-      vs_wait(cx, 0);   VT(25);
-      vs_accumulate(D0 + c16, cur.pw[1], s1, s2);
-      VT(26);
-   
-      // ================= round 7
-      // view 2's last stage moves to stream A (idle since round 6): its input goes to A's activation columns; stream B is then
-      // free for view 0 of the next tile while that stage runs
-      vs_wait(cx, 1);   VT(27);
-      vs_epi_sp(D1 + c32, A0 + c16, cq == 3);
-      vs_signal(cx, 0, lane);   VT(28);
-      prev_id = cur.id; prev_si = cur.si; prev_live = cur.live; prev_pw2 = cur.pw[2];
-      prev_s0 = (cur.pw[0] + cur.pw[1]) + cur.pw[2];
-      if (it < nreal) { start_tile(it + 1);   VT(29); }
-    }
-#ifdef KPN_STAGE_TIMING
-    if ((int)blockIdx.x == tim_blk && warp == 0 && lane == 0) { kpn_tim_tile[0] = min(nreal + 1, TIM_TILES); kpn_tim_tile[1] = kpn_tim_tile[0]; }
-#endif
-    vs_wait(cx, 0);   // the last (ghost) view-2 stage: tensor memory must be idle before it is released
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-#ifdef KPN_STAGE_TIMING
-  if (t == 0 && blockIdx.x < 256) kpn_tim[3 * TIM_TILES * TIM_WORDS + blockIdx.x] = (unsigned long long)(clock64() - blk_t0);
-#endif
-  tc::cluster_sync_all();
-  if (warp == 0) tc::tmem_dealloc2(tbase, 512);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// colour kernel
-// ------------------------------------------------------------------------------------------------------------------
-template <int NK>
-__global__ void __launch_bounds__(TCC_THREADS, 1)
+__global__ void __launch_bounds__(CWG * 128, 1)
 shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wblob,
                    SampleSrc src, const int2* __restrict__ list2, const int* __restrict__ list1,
                    const int* __restrict__ count_ptr, const uint4* __restrict__ lat_in, int query_mode, ShadeOut so) {
   extern __shared__ __align__(1024) uint8_t wsm[];
-  __shared__ uint64_t bars[1 + 2 * CSLOT];   // [0] weights | per slot: a_ready, acc_ready
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t wbar;
   __shared__ SceneS scs;
   constexpr TcPlan plan = make_tc_plan(NK);
   constexpr uint32_t OFF0 = plan.st[GEO_NSTAGE].off, WBYTES = plan.total_bytes - plan.st[GEO_NSTAGE].off;
-  const int t = threadIdx.x, warp = __shfl_sync(FULL, t >> 5, 0), lane = t & 31;   // warp-uniform (see shade_geo_kernel)
+  constexpr uint32_t WPAD = (WBYTES + 1023u) / 1024u * 1024u;
+  const int t = threadIdx.x, wg = t >> 7;
   const int count = *count_ptr;
   const int ntiles = (count + SPT - 1) / SPT;
-  stage_scene(scs, *scp, NK, t, TCC_THREADS);
-  if (warp == 0) tc::tmem_alloc(&tmem_base_s, 512);
-  if (t == 0) {
-    tc::mbar_init(&bars[0], 1);
-    for (int s = 0; s < CSLOT; ++s) { tc::mbar_init(&bars[1 + 2 * s], ROW_WARPS); tc::mbar_init(&bars[2 + 2 * s], 1); }
-    tc::fence_mbar_init();
-  }
+  if (blockIdx.x * CWG >= ntiles) return;
+  stage_scene(scs, *scp, NK, t, CWG * 128);
+  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
   __syncthreads();
-  if (t == 0 && ntiles > 0) load_weights(wsm, wblob + OFF0, WBYTES, &bars[0]);   // the colour stages' weight tiles, once per CTA
-  tc::fence_before_sync();
+  if (t == 0) load_weights(wsm, wblob + OFF0, WBYTES, &wbar);   // the colour stages' weight tiles, once per CTA
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-  {
-    const int slot = warp / ROW_WARPS, roww = warp % ROW_WARPS;
-    RowCtx cx;
-    const uint32_t tm = tbase + (uint32_t)slot * 128u + ((uint32_t)(roww * 32) << 16);
-    cx.R0 = tm; cx.R1 = tm + 64u;
-    cx.a_ready = &bars[1 + 2 * slot];
-    cx.acc_ready = &bars[2 + 2 * slot];
-    cx.ph = 0;
-    cx.issuer = roww == 0 ? 1 : 0;
-    cx.pha = 0;
-    cx.slot_tm = tbase + (uint32_t)slot * 128u;
-    cx.wlo0 = (tc::smem_u32(wsm) >> 4) & 0x3FFFu;
-    cx.el = tc::elect_one();
-    cx.gb = 3 * (lane / 3);
-    cx.l1 = (cx.gb + (lane - cx.gb + 1) % 3) & 31;
-    cx.l2 = (cx.gb + (lane - cx.gb + 2) % 3) & 31;
-    for (int tile = blockIdx.x * CSLOT + slot; tile < ntiles; tile += gridDim.x * CSLOT)
-      color_tile<NK>(scs, C, src, list2, list1, count, tile, cx, roww, lane, lat_in, query_mode, so);
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, 512);
+  const int lane = t & 31;
+  ColCtx cx{wsm + WPAD + (size_t)wg * (CA_BYTES + CD_BYTES), nullptr, tc::smem_u32(wsm), 1 + wg, t & 127, (t >> 5) & 3, lane,
+            Group(lane)};
+  cx.D = reinterpret_cast<float*>(cx.A + CA_BYTES);
+  for (int tile = blockIdx.x * CWG + wg; tile < ntiles; tile += gridDim.x * CWG)
+    color_tile<NK>(scs, C, src, list2, list1, count, tile, cx, lat_in, query_mode, so);
 }
 
 }  // namespace
 
 size_t tc_weight_blob_bytes(int n_kpt) { return make_tc_plan(n_kpt).total_bytes; }
-size_t tc_weight_lo_bytes(int n_kpt) { return make_tc_plan(n_kpt).st[TC_NLO].off; }
+size_t tc_weight_lo_bytes(int n_kpt) {
+  const TcPlan p = make_tc_plan(n_kpt);
+  return p.st[GEO_NSTAGE].off - p.st[4].off;
+}
+size_t tc_pool_bytes(long long n_max) { return (size_t)(n_max < POOL_SLICE ? n_max : POOL_SLICE) * POOL_W * sizeof(float); }
 bool tc_supported(int n_views, int n_kpt, int sp_level) { return n_views == 3 && (n_kpt == 18 || n_kpt == 24) && sp_level == 3; }
 
-template <int NK, bool VSEQ = false>
-static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wpair, int two_term,
+template <int NK>
+static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask,
                                   const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                                  const ShadeOut& so, uint4* lat, int2* list2, int* count2, int num_sms, cudaEvent_t after_geo, cudaStream_t st) {
+                                  const ShadeOut& so, uint4* lat, float* pool, int2* list2, int* count2, int num_sms,
+                                  cudaEvent_t after_geo, int* launches, cudaStream_t st) {
   constexpr TcPlan plan = make_tc_plan(NK);
-  const size_t smem_geo = plan.st[GEO_NSTAGE].off + (geo_pref(NK) ? (size_t)NSLOT * GEO_FW * 128 * 4 : 0);
-  const size_t smem_col = plan.total_bytes - plan.st[GEO_NSTAGE].off;
-  const size_t smem_vs = plan.st[GEO_NSTAGE].off + VS_STAGING_BYTES;
+  const size_t smem_front = plan.st[4].off + (size_t)GWG * front_tile_bytes(NK);
+  const size_t smem_tail = 2 * (size_t)(plan.st[GEO_NSTAGE].off - plan.st[4].off) + (size_t)GWG * TAIL_TILE_BYTES;
+  const size_t smem_col = (plan.total_bytes - plan.st[GEO_NSTAGE].off + 1023) / 1024 * 1024 + (size_t)CWG * (CA_BYTES + CD_BYTES);
   static std::atomic<bool> attr[64];   // function attributes are per device (zero-initialised; setting them twice is harmless)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(shade_geo_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_geo);
+    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
     if (e != cudaSuccess) return e;
-    if constexpr (VSEQ) {
-      e = cudaFuncSetAttribute(shade_geo_vseq_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_vs);
-      if (e != cudaSuccess) return e;
-    }
+    e = cudaFuncSetAttribute(geo_tail_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
+    if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(shade_color_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_col);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
-  const long long max_tiles = (n_max + SPT - 1) / SPT;
-  long long pairs = (max_tiles + 2 * NSLOT - 1) / (2 * NSLOT);   // clusters that can have work
-  const int max_clusters = num_sms / 2;
-  int grid = 2 * (int)(pairs < 1 ? 1 : (pairs > max_clusters ? max_clusters : pairs));
-  static const int relaxed_arrive = [] { const char* e = getenv("KPN_RELAXED_ARRIVE"); return e && e[0] == '0' ? 0 : 1; }();
-  // which stages get the W_lo pass (bits 0..5) and the A_lo pass (bits 6, 7 for stages 4, 5); KPN_LO_MASK overrides (experiments)
-  static const int lo_env = [] { const char* e = getenv("KPN_LO_MASK"); return e ? (int)strtol(e, nullptr, 0) : -1; }();
-  two_term = two_term ? (lo_env >= 0 ? lo_env : 0xFF) : 0xC0;
-  if constexpr (VSEQ) {
-    const long long vt = (n_max + 127) / 128;
-    long long vp = (vt + 1) / 2;
-    const int vgrid = 2 * (int)(vp < 1 ? 1 : (vp > max_clusters ? max_clusters : vp));
-#ifdef KPN_STAGE_TIMING   // instrumented build only: producers skip the gathers (garbage output; measures the pipeline's floor)
-    static const int fake = [] {   // bits 0-7: KPN_VS_FAKE; bits 8+: the block whose warps are stamped (KPN_TIM_BLOCK, even = leader CTA)
-      const char* e = getenv("KPN_VS_FAKE");
-      const char* b = getenv("KPN_TIM_BLOCK");
-      return (e && e[0] == '1' ? 1 : 0) | ((b ? atoi(b) : 0) << 8);
-    }();
-#else
-    const int fake = 0;
-#endif
-    shade_geo_vseq_kernel<NK><<<vgrid, VS_THREADS, smem_vs, st>>>(sc, C, wpair, two_term, src, list, counter, query_mode, so, lat, fake);
-  } else {
-    shade_geo_kernel<NK><<<grid, GEO_THREADS, smem_geo, st>>>(sc, C, wpair, two_term, src, list, counter, query_mode, so, lat,
-                                                             relaxed_arrive);
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
-  long long g = (max_tiles + CSLOT - 1) / CSLOT;
-  grid = (int)(g < 1 ? 1 : (g > num_sms ? num_sms : g));
-  if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
-    shade_color_kernel<NK><<<grid, TCC_THREADS, smem_col, st>>>(sc, C, wblob, src, nullptr, list, counter, lat, query_mode, so);
+  auto grid_for = [&](long long tiles, int per_cta) {
+    const long long g = (tiles + per_cta - 1) / per_cta;
+    return (int)(g < 1 ? 1 : (g > num_sms ? num_sms : g));
+  };
+  cudaError_t e = cudaSuccess;
+  // the device-side count is not known here: every slice of [0, n_max) is launched, slices past the count exit at once
+  const long long nslices = n_max > POOL_SLICE ? (n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
+  for (long long s = 0; s < nslices; ++s) {
+    const long long base = s * POOL_SLICE, len = n_max - base < POOL_SLICE ? n_max - base : POOL_SLICE;
+    geo_front_kernel<NK><<<grid_for((len + FSPT - 1) / FSPT, GWG), GWG * 128, smem_front, st>>>(sc, wblob, src, list, counter, base,
+                                                                                                  len, pool);
+    geo_tail_kernel<NK><<<grid_for((len + 63) / 64, GWG), GWG * 128, smem_tail, st>>>(C, wblob, wlo, lo_mask, list, counter, base,
+                                                                                       len, pool, query_mode, so, lat);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+    *launches += 2;
+  }
+  if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
+  const int grid = grid_for((n_max + SPT - 1) / SPT, CWG);
+  if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
+    shade_color_kernel<NK><<<grid, CWG * 128, smem_col, st>>>(sc, C, wblob, src, nullptr, list, counter, lat, query_mode, so);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    *launches += 1;
     return cudaMemcpyAsync(count2, counter, sizeof(int), cudaMemcpyDeviceToDevice, st);   // statistics: every valid sample was coloured
   }
   const long long lb = (n_max + 1023) / 1024;
-  colour_list_kernel<<<(int)(lb < 1 ? 1 : (lb > 148 * 8 ? 148 * 8 : lb)), 256, 0, st>>>(list, counter, so.ao, so.list_base, list2, count2);
+  colour_list_kernel<<<(int)(lb < 1 ? 1 : (lb > num_sms * 8 ? num_sms * 8 : lb)), 256, 0, st>>>(list, counter, so.ao, so.list_base,
+                                                                                                 list2, count2);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  shade_color_kernel<NK><<<grid, TCC_THREADS, smem_col, st>>>(sc, C, wblob, src, list2, nullptr, count2, lat, query_mode, so);
+  shade_color_kernel<NK><<<grid, CWG * 128, smem_col, st>>>(sc, C, wblob, src, list2, nullptr, count2, lat, query_mode, so);
+  *launches += 2;
   return cudaGetLastError();
 }
 
-cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wpair, int two_term, int n_kpt,
+cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term, int n_kpt,
                             const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                            const ShadeOut& so, void* lat_scratch, void* list2, int* count2, int num_sms, cudaEvent_t after_geo,
-                            cudaStream_t st) {
-  if (n_kpt == -18)   // view-sequential geometry kernel (kpn_api.cu negates n_kpt to select it)
-    return launch_tc_impl<18, true>(sc, C, wblob, wpair, two_term, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
-                                    (int2*)list2, count2, num_sms, after_geo, st);
+                            const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
+                            cudaEvent_t after_geo, int* launches, cudaStream_t st) {
+  // W_lo and A_lo passes of the density tail (stages 4, 5: bits 4, 5 and 6, 7); single-term weights keep the A_lo passes
+  const int lo_mask = two_term ? 0xF0 : 0xC0;
   if (n_kpt == 18)
-    return launch_tc_impl<18>(sc, C, wblob, wpair, two_term, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
-                              (int2*)list2, count2, num_sms, after_geo, st);
-  return launch_tc_impl<24>(sc, C, wblob, wpair, two_term, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
-                            (int2*)list2, count2, num_sms, after_geo, st);
+    return launch_tc_impl<18>(sc, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
+                              (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo, launches, st);
+  return launch_tc_impl<24>(sc, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
+                            (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo, launches, st);
 }
 
 // Watchdog state of this module's kernels: out[0] != 0 -> some barrier wait gave up at block out[1], thread out[2], tag out[3].
@@ -1931,26 +915,10 @@ cudaError_t tc_watchdog_clear_async(cudaStream_t st) {
   return cudaMemsetAsync(p, 0, 8 * sizeof(unsigned int), st);
 }
 
-// stage-timing dump of the instrumented build (KPN_STAGE_TIMING); returns cudaErrorNotSupported otherwise
+// stage-timing instrumentation is not built for this architecture's kernels
 cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles) {
-#ifdef KPN_STAGE_TIMING
-  cudaError_t e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) return e;
-  int nt[2] = {0, 0};
-  e = cudaMemcpyFromSymbol(nt, kpn_tim_tile, sizeof(nt));
-  if (e != cudaSuccess) return e;
-  *n_tiles = nt[0] < nt[1] ? nt[0] : nt[1];
-  const size_t bytes = sizeof(unsigned long long) * (size_t)(n_words < 3 * TIM_TILES * TIM_WORDS + 256 ? n_words : 3 * TIM_TILES * TIM_WORDS + 256);
-  e = cudaMemcpyFromSymbol(out, kpn_tim, bytes);
-  if (e != cudaSuccess) return e;
-  const int zero[2] = {0, 0};
-  return cudaMemcpyToSymbol(kpn_tim_tile, zero, sizeof(zero));
-#else
   (void)out; (void)n_words; (void)n_tiles;
   return cudaErrorNotSupported;
-#endif
 }
-
-size_t tc_pair_blob_bytes(int n_kpt) { return 2 * (size_t)make_tc_plan(n_kpt).st[GEO_NSTAGE].off; }
 
 }  // namespace kpn

@@ -1,7 +1,6 @@
-// Thin inline-PTX layer over the sm_100a tensor-core path: TMEM allocation, tcgen05.mma (A operand in
-// TMEM, B operand in shared memory through a matrix descriptor), tcgen05.ld/st, tcgen05.commit, mbarrier
-// and the 1-D bulk (TMA) copy.  Encodings follow the PTX ISA tcgen05 chapter; the bit layouts of the
-// shared-memory and instruction descriptors are restated in the comments below.
+// Thin inline-PTX layer over the sm_90a tensor-core path: warpgroup MMA (wgmma.mma_async, both operands in shared memory
+// through matrix descriptors, fp32 accumulators in registers), mbarrier and the 1-D bulk (TMA) copy.  Encodings follow the
+// PTX ISA wgmma chapter; the bit layout of the shared-memory descriptor is restated below.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -85,191 +84,48 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 // generic-proxy writes to shared memory -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM allocation (warp-wide, one warp owns alloc and dealloc) --------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // ---- descriptors ---------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit), K-major operand, no swizzle ("interleaved" core matrices of
-// 8 rows x 16 bytes stored as 128 contiguous bytes):
-//   [0,14)  start address >> 4      [16,30) leading-dimension byte offset >> 4 (distance between the two
-//   [32,46) stride-dimension byte offset >> 4 (distance between 8-row groups)   core matrices along K)
-//   [46,48) version = 1 (sm_100)    [61,64) layout/swizzle type = 0 (none)
+// Shared-memory matrix descriptor (64 bit), K-major operand, no swizzle ("interleaved" core matrices of 8 rows x 16 bytes
+// stored as 128 contiguous bytes):
+//   [0,14)  start address >> 4      [16,30) leading-dimension byte offset >> 4 (distance between core matrices along K)
+//   [32,46) stride-dimension byte offset >> 4 (distance between 8-row groups)   [62,64) swizzle mode = 0 (none)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// Instruction descriptor (32 bit) for kind::f16, fp16 A/B (both K-major), fp32 accumulate:
-//   [4,6) D format = 1 (F32)   [7,10) A format = 0 (F16)   [10,13) B format = 0 (F16)
-//   [15] A major = 0 (K)  [16] B major = 0 (K)  [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// ---- warpgroup MMA ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+}  // namespace tc
+}  // namespace kpn
+#include "kpn_wgmma.cuh"
+namespace kpn {
+namespace tc {
+
+// An activation tile of ROWS rows in shared memory, K-major core matrices in the order [k/8][row/8][row%8][k%8] (fp16):
+// LBO = (ROWS/8) * 128 bytes, SBO = 128 bytes.  Byte offset of 32-bit word column c (fp16 elements 2c, 2c+1) of row r.
+template <int ROWS>
+__host__ __device__ constexpr uint32_t a_word_off(int r, int c) {
+  return (uint32_t)((((c >> 2) * (ROWS >> 3) + (r >> 3)) * 128) + (r & 7) * 16 + (c & 3) * 4);
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]^T ; one elected thread issues.  M = 128, K = 16 per instruction.
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when every previously issued tcgen05.mma of this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// D[64 x N] (+)= A[64 x 16*KCH] * B[N x 16*KCH]^T for the warpgroup's 64-row tile at `a_addr` (activation layout above with
+// a_lbo = (tile rows / 8) * 128) and a weight tile at `b_addr` ([k/8][n/8][8][8], LBO = (Np/8)*128).  `acc` = 0 overwrites d.
+// The caller brackets a chain of these with wg_fence() / wg_commit() + wg_wait0().
+template <int N, int KCH>
+__device__ __forceinline__ void wg_mma(float* d, uint32_t a_addr, uint32_t a_lbo, uint32_t b_addr, uint32_t b_lbo, uint32_t acc) {
+#pragma unroll
+  for (int j = 0; j < KCH; ++j)
+    Wgmma<N>::mma(d, make_smem_desc(a_addr + 2u * a_lbo * (uint32_t)j, a_lbo, 128u),
+                  make_smem_desc(b_addr + 2u * b_lbo * (uint32_t)j, b_lbo, 128u), (acc || j > 0) ? 1u : 0u);
 }
 
-// ---- CTA-pair (cta_group::2) variants: both CTAs of a 2-CTA cluster take part, the leader (cluster rank 0) issues ----
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {   // one warp in EACH CTA, same smem offset
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[256 x N] (+)= A[256 x 16] * B[N x 16]^T : rows 0..127 of A/D live in the leader's TMEM, 128..255 in the peer's (same
-// column addresses); each CTA holds N/2 rows of B at the same shared-memory offset.
-__device__ __forceinline__ void mma_ts2(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: arrive on the mbarrier at this shared offset in BOTH CTAs once all prior MMAs of this thread completed
-__device__ __forceinline__ void mma_commit2(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// arrive on the mbarrier at the same shared offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-
-// ---- TMEM <-> registers: 32 lanes x 32 bit, each thread touches its own lane (= tile row) ----------------
-// taddr: bits [31:16] lane, [15:0] column.  A warp may only touch lanes 32*(warp_id%4) .. +31.
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-
-// ---- warp-converged issue: every lane runs the issue code (operands stay in uniform registers), one elected lane's
-//      instruction takes effect.  `el` = 1 in the elected lane (elect.sync picks the same lane for a given member mask).
-__device__ __forceinline__ uint32_t elect_one() {
-  uint32_t p;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(p));
-  return p;
-}
-// CTA-pair MMA with the shared-memory descriptor given as two 32-bit halves (the high half is a per-kernel constant, the
-// low half advances by a compile-time step per K chunk) and an issue predicate.
-__device__ __forceinline__ void mma_ts2_el(uint32_t d_tmem, uint32_t a_tmem, uint32_t desc_lo, uint32_t desc_hi, uint32_t idesc,
-                                           uint32_t accumulate, uint32_t el) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 bd;\n\tsetp.ne.b32 p, %5, 0;\n\tsetp.ne.b32 q, %6, 0;\n\tmov.b64 bd, {%2, %3};\n\t"
-      "@q tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], bd, %4, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(desc_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate), "r"(el)
-      : "memory");
-}
-// single-CTA variants of the warp-converged issue
-__device__ __forceinline__ void mma_ts_el(uint32_t d_tmem, uint32_t a_tmem, uint32_t desc_lo, uint32_t desc_hi, uint32_t idesc,
-                                          uint32_t accumulate, uint32_t el) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 bd;\n\tsetp.ne.b32 p, %5, 0;\n\tsetp.ne.b32 q, %6, 0;\n\tmov.b64 bd, {%2, %3};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], bd, %4, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "r"(desc_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate), "r"(el)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_el(uint64_t* bar, uint32_t el) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar)), "r"(el)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit2_el(uint64_t* bar, uint32_t el) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t"
-      "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(smem_u32(bar)),
-      "h"((uint16_t)3), "r"(el)
-      : "memory");
-}
 // named barriers (ids 1..15): producer arrives, consumer syncs; `count` = threads of both sides
 __device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }

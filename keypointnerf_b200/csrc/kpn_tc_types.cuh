@@ -1,5 +1,5 @@
-// Tensor-core engine: stage table (which dense layers run on tcgen05, their padded shapes and where their
-// fp16 weights sit in the shared-memory blob) and the fp32 constants that travel as kernel parameters
+// Tensor-core engine: stage table (which dense layers run on the tensor cores, their padded shapes and where their
+// fp16 weights sit in the weight blob) and the fp32 constants that travel as kernel parameters
 // (biases of the tensor-core layers + the tiny layers that stay on the CUDA cores in fp32).
 #pragma once
 #include <stdint.h>
@@ -13,7 +13,7 @@ constexpr int TC_NSTAGE = 13;
 // Stage 12 (second ray-encoder layer 16->35 of the colour head, executed FIRST in the colour kernel) also carries its bias row.
 // The geometry stages (0..5) carry their bias as one extra K row (the activation tile holds a constant 1 there), so their
 // epilogues have no per-column constants.  Stage 0 additionally permutes its inputs (tc_kmap) so that the two threads
-// that build a row's input each write one contiguous, naturally aligned run of tensor-memory columns.
+// that build a row's input each write one contiguous, 16-byte aligned run of activation-tile columns.
 
 struct TcStage {
   int Kp, Np;
@@ -60,26 +60,6 @@ __host__ __device__ constexpr int tc_kbias(int stage, int n_kpt) {
     default: return 64;
   }
 }
-
-// ---- "view-sequential" geometry kernel (18 keypoints; engines 0 and 3): a row is a SAMPLE, its three views are run through
-// stages 0-3 one after the other, FOUR threads build / post-process a row (column quarters).  Layer-0 input of one
-// (sample, view): 96 packed columns = 4 runs of 24: threads 0-2: two keypoint pairs (14 columns) + five float4 groups of feat64
-// (10 columns); thread 3: three pairs (21) + one group (2) + the bias column.
-__host__ __device__ constexpr int vs_run_cols(int n_kpt) { return n_kpt == 18 ? 24 : 0; }
-__host__ __device__ constexpr int tc_kmap_vseq(int stage, int n_kpt, int i) {
-  if (stage != 0) return i;
-  if (i < 7 * n_kpt) {
-    const int r = i / n_kpt, k = i % n_kpt, j = k / 2;
-    const int t = j < 6 ? j / 2 : 3;
-    const int col = 24 * t + (j < 6 ? (j % 2) * 7 : (j - 6) * 7) + r;
-    return 2 * col + (k & 1);
-  }
-  const int c = i - 7 * n_kpt, g = c / 4;
-  const int t = g < 15 ? g / 5 : 3, gi = g < 15 ? g % 5 : 0;
-  const int col = 24 * t + (t < 3 ? 14 : 21) + 2 * gi + (c % 4) / 2;
-  return 2 * col + (c & 1);
-}
-__host__ __device__ constexpr int tc_kbias_vseq(int stage, int n_kpt) { return stage == 0 ? 2 * 95 : tc_kbias(stage, n_kpt); }
 
 __host__ __device__ constexpr TcPlan make_tc_plan(int n_kpt) {
   TcPlan p{};

@@ -241,7 +241,7 @@ class KeypointNeRF(nn.Module):
         """Arithmetic type of the dense layers in the selected engine."""
         sp = self.sp_encoder
         tc = self.engine != 1
-        return "fp16 operands, fp32 accumulate (tcgen05)" if tc else "fp32"
+        return "fp16 operands, fp32 accumulate (wgmma)" if tc else "fp32"
 
     def _bind_scene(self, cam, feat_geo, feat_tex, sp_data, img, fg_mask, bounds):
         m = self.marcher()

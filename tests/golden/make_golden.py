@@ -26,6 +26,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.abspath(os.path.join(HERE, "..", "..")))
 from keypointnerf_b200 import synthetic as syn  # noqa: E402
+from tests.util import save_golden  # noqa: E402
 
 
 def _stub(name, **attrs):
@@ -230,7 +231,10 @@ def main():
         meta = {k: v for k, v in c.items() if k != "capture"}
         res["input_sha256"] = np.frombuffer(checksum(scene, weights).encode(), dtype=np.uint8)
         res["meta"] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
-        np.savez_compressed(os.path.join(HERE, name + ".npz"), **res)
+        res.pop("rgba_fine", None)          # no test reads them
+        if not c["fine"]:
+            res.pop("z_coarse", None)
+        save_golden(name, res, HERE)
         print(name, res["tex_fg"].shape, "valid frac", valid_frac, "alpha mean", float(res["alpha"].mean()),
               "alpha max", float(res["alpha"].max()), flush=True)
 

@@ -3,8 +3,8 @@ against (a) golden vectors produced by the reference itself and (b) the CPU orac
 seeded inputs.
 
 Gate (BASELINE.json north_star): RGB within 1e-3 abs of the reference, PSNR delta < 0.01 dB.
-  * engines 0 and 4 (tcgen05, fp16 operands with two-term weights, fp32 accumulate; 0 runs the view-sequential geometry kernel at
-    18 keypoints, 4 the row-per-view one everywhere) are held to exactly that on RGB, on EVERY ray;
+  * engines 0 and 4 (wgmma tensor cores, fp16 operands with a two-term density tail, fp32 accumulate; 4 is an alias of 0 that
+    selected a second geometry kernel on an earlier architecture) are held to exactly that on RGB, on EVERY ray;
     accumulated alpha / per-sample compositing weights / depth are looser by the factors below (they are
     not averaged by colours in [0,1] and the density head has a x30 gain in the synthetic recipe);
   * engine 1 (fp32 CUDA cores) is held to fp32 round-off.
@@ -26,7 +26,7 @@ from tests.util import checksum, load_golden, psnr, scene_from_meta
 
 pytestmark = pytest.mark.gpu
 
-ENGINES = [0, 1, 4]   # default (view-sequential geometry kernel at 18 keypoints), fp32 CUDA cores, row-per-view geometry kernel
+ENGINES = [0, 1, 4]   # default tensor-core engine, fp32 CUDA cores, engine 4 (same kernels as 0)
 TOL = {
     0: dict(rgb=1e-3, alpha=3e-3, contrib=3e-3, depth=3e-2, sdf=3e-2, q99_fine=2.5e-3, psnr=70.0),
     1: dict(rgb=1e-4, alpha=1e-4, contrib=1e-4, depth=2e-3, sdf=2e-3, q99_fine=1e-3, psnr=80.0),
@@ -396,7 +396,7 @@ def test_full_frame_properties_at_baseline_size():
     e_rob = float(err[~flipped].max())
     mse = float(((frame["tex_fg"] - ref["tex_fg"]) ** 2)[:, ~flipped].mean())
     p = 10 * np.log10(1.0 / mse)
-    print(f"512^2x128 frame, tcgen05 vs fp32 engine: max rgb err {e_rob:.2e} on {1 - frac_flipped:.4f} of rays, psnr {p:.1f} dB; "
+    print(f"512^2x128 frame, tensor-core vs fp32 engine: max rgb err {e_rob:.2e} on {1 - frac_flipped:.4f} of rays, psnr {p:.1f} dB; "
           f"final-sample step flips on {frac_flipped:.4%} of rays")
     assert e_rob < 1e-3 and p > 60.0 and frac_flipped < 0.01
 
@@ -424,7 +424,7 @@ def test_24_keypoint_frame_many_tiles_per_slot():
     flipped = (frame["alpha"] - ref["alpha"]).abs() > 0.05
     err = (frame["tex_fg"] - ref["tex_fg"]).abs().amax(0)
     e_rob = float(err[~flipped].max())
-    print(f"24-keypoint 192^2x96 frame, tcgen05 vs fp32 engine: max rgb err {e_rob:.2e}, flipped {float(flipped.float().mean()):.4%}")
+    print(f"24-keypoint 192^2x96 frame, tensor-core vs fp32 engine: max rgb err {e_rob:.2e}, flipped {float(flipped.float().mean()):.4%}")
     assert e_rob < 1e-3 and float(flipped.float().mean()) < 0.01
 
 

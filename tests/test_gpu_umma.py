@@ -1,5 +1,5 @@
-"""tcgen05 primitive self-test: one 128 x N x K fp16 tile (fp32 accumulate) against torch.matmul for
-every (N, K) the network kernels use, with the A operand staged in tensor memory."""
+"""Tensor-core primitive self-test: one 128 x N x K fp16 tile (fp32 accumulate) through wgmma against torch.matmul for
+every (N, K) the network kernels use, with the A operand in the activation-tile layout the kernels' epilogues write."""
 import pytest
 import torch
 
@@ -28,7 +28,7 @@ def test_umma_tile(N, K, variant):
     assert err < 2e-3, f"variant {variant} N={N} K={K}: max err {err}"
 
 
-# (N, K, a_col, d_col): the geometry kernel's stage shapes and tensor-memory placements (kpn_shade_tc.cu geo_dcol)
+# (N, K, a_col, d_col): stage shapes of the geometry network, A placed at column a_col of a d_col-column activation tile
 PAIR_CASES = [(128, 192, 0, 128), (128, 240, 0, 128), (128, 144, 0, 128), (64, 128, 0, 192), (96, 144, 0, 160),
               (96, 128, 64, 160), (64, 80, 0, 128), (64, 64, 32, 128), (32, 32, 8, 256), (96, 16, 128, 160)]
 
@@ -36,8 +36,8 @@ PAIR_CASES = [(128, 192, 0, 128), (128, 240, 0, 128), (128, 144, 0, 128), (64, 1
 @pytest.mark.parametrize("mode", [0, 1, 2])
 @pytest.mark.parametrize("N,K,a_col,d_col", PAIR_CASES)
 def test_umma_cta_pair_tile(N, K, a_col, d_col, mode):
-    """cta_group::2: one 256 x N x K tile on a 2-CTA cluster, each CTA holding half of B's rows; activation tile and
-    accumulator at the column offsets the geometry kernel uses; single-thread and warp-converged (elected lane) issue."""
+    """One 256 x N x K tile on a 2-CTA cluster, each CTA holding half of B's rows and fetching the other half from its peer's
+    shared memory (mode 0: remote reads, 1: bulk copy completing on an mbarrier, 2: remote stores) before its wgmma."""
     lib = L.load()
     g = torch.Generator(device="cpu").manual_seed(N * 1000 + K + 7)
     A = (torch.randn(256, K, generator=g) * 0.5).half().cuda()

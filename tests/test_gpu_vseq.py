@@ -1,5 +1,5 @@
-"""Engine 3 (the view-sequential geometry kernel requested explicitly; engine 0 selects it at 18 keypoints): same gates as
-tests/test_gpu_parity.py, against the reference's goldens, the fp32 engine and the row-per-view kernel (engine 4)."""
+"""Engine 3 (an alias of the default tensor-core engine; it selected a view-sequential geometry kernel on an earlier
+architecture): same gates as tests/test_gpu_parity.py, against the reference's goldens, the fp32 engine and engine 4."""
 import numpy as np
 import pytest
 import torch

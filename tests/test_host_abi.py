@@ -97,7 +97,7 @@ def test_product_never_imports_oracle():
 def test_tensor_core_input_permutation_is_a_bijection(lib, n_kpt):
     """Geometry-stage weight packing (host code of the library, no GPU): every input of a stage is multiplied with its own K
     index, the bias row has a K index of its own, everything fits the padded K; layer 0 additionally keeps the two column runs
-    (thread 0 | thread 1) 8-column aligned as the tensor-memory stores of the kernel require."""
+    (thread 0 | thread 1) aligned as the activation-tile stores of the kernel require."""
     n_in = {0: 7 * n_kpt + 64, 1: 128, 2: 136, 3: 120, 4: 128, 5: 64}
     for stage, n in n_in.items():
         kmap = (C.c_int * n)()

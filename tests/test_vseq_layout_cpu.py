@@ -1,9 +1,10 @@
-"""Host-side checks of two contracts of the view-sequential geometry kernel (keypointnerf_b200/csrc/kpn_shade_tc.cu) that a GPU run
-would only show as a slowdown or as a subtle numerical drift:
+"""Host-side checks of two contracts of the tensor-core kernels (keypointnerf_b200/csrc/kpn_shade_tc.cu, kpn_tc.cuh) that a GPU
+run would only show as a slowdown or as a subtle numerical drift:
 
-  * the shared-memory staging layout `vs_f64_word` (producers write eight float4 groups of a row from eight adjacent lanes, the row
-    warps read one word of 32 consecutive rows): a bijection per word, and free of bank conflicts on both sides;
-  * the thread-local view pooling: mean = S1, var = S2 - S1^2 (2 - sum pw) with S1 = sum pw x, S2 = sum pw x^2 is the reference's
+  * the shared-memory activation-tile layout `a_word_off` (row threads store 16-byte runs of their row, 32 consecutive rows per
+    warp; the accumulator epilogues store one word per lane from the wgmma fragment): a bijection, and free of bank conflicts on
+    both sides;
+  * the view pooling identity: mean = S1, var = S2 - S1^2 (2 - sum pw) with S1 = sum pw x, S2 = sum pw x^2 is the reference's
     weighted mean / variance (reference src/utils.py:722-748, restated in oracle/kpnerf_oracle.py) for weights that do NOT sum to 1
     exactly (they are normalised with a 1e-6 guard, reference src/model.py:757-759).
 """
@@ -13,38 +14,40 @@ import re
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = open(os.path.join(ROOT, "keypointnerf_b200", "csrc", "kpn_shade_tc.cu")).read()
+SRC = open(os.path.join(ROOT, "keypointnerf_b200", "csrc", "kpn_tc.cuh")).read()
+SHADE = open(os.path.join(ROOT, "keypointnerf_b200", "csrc", "kpn_shade_tc.cu")).read()
 
 
-def vs_f64_word(w, row):
-    return w * 128 + (row ^ (4 * ((w >> 1) & 7)))
+def a_word_off(rows, r, c):
+    return (((c >> 2) * (rows >> 3) + (r >> 3)) * 128) + (r & 7) * 16 + (c & 3) * 4
 
 
 def test_python_restatement_matches_the_source():
-    m = re.search(r"int vs_f64_word\(int w, int row\) \{ return (.*?); \}", SRC)
-    assert m, "vs_f64_word not found"
-    assert m.group(1).replace(" ", "") == "w*128+(row^(4*((w>>1)&7)))"
-    # the producers' store address is the same function written out for words 2g, 2g+1, 2g+16, 2g+17 of group pair (g, 8+g)
-    assert "f64b + (2 * l8) * 128 + (row ^ (4 * l8))" in SRC
-    assert "d[16 * 128] = w0; d[17 * 128] = w1;" in SRC
+    m = re.search(r"a_word_off\(int r, int c\) \{\s*return \(uint32_t\)\((.*?)\);\s*\}", SRC, re.S)
+    assert m, "a_word_off not found"
+    assert m.group(1).replace(" ", "") == "(((c>>2)*(ROWS>>3)+(r>>3))*128)+(r&7)*16+(c&3)*4"
+    # the fragment epilogues address pair m of the accumulator as row 16*wq + lane/4 + 8*(m&1), word 4*(m>>1) + lane%4
+    assert "const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);" in SHADE
 
 
 def test_staging_words_are_a_bijection_per_word():
-    for w in range(32):
-        idx = {vs_f64_word(w, r) for r in range(128)}
-        assert idx == set(range(w * 128, (w + 1) * 128))
+    for rows, words in ((64, 120), (128, 56)):
+        idx = {a_word_off(rows, r, c) for r in range(rows) for c in range(words)}
+        assert len(idx) == rows * words and max(idx) == rows * words * 4 - 4 and all(i % 4 == 0 for i in idx)
 
 
 def test_no_bank_conflicts_on_either_side():
-    # consumer: lanes = 32 consecutive rows of one lane quarter, one word
-    for w in range(32):
-        for q4 in range(4):
-            banks = {vs_f64_word(w, 32 * q4 + lane) % 32 for lane in range(32)}
-            assert len(banks) == 32
-    # producer: one store instruction of a warp = lanes (row 4u + l/8, group g = l%8), word 2g + i for fixed i in {0, 1, 16, 17}
-    for u in range(32):
-        for i in (0, 1, 16, 17):
-            banks = {vs_f64_word(2 * (lane % 8) + i, 4 * u + lane // 8) % 32 for lane in range(32)}
+    for rows in (64, 128):
+        # row threads: one 16-byte store per lane of 32 consecutive rows (run start c % 4 == 0), served per quarter warp
+        for r0 in range(0, rows, 32):
+            for c in range(0, 64, 4):
+                for q in range(4):
+                    banks = {(a_word_off(rows, r0 + 8 * q + i, c) // 4 + j) % 32 for i in range(8) for j in range(4)}
+                    assert len(banks) == 32
+    # accumulator epilogue (64-row tiles): one word per lane, pair m of the fragment of row warp wq
+    for wq in range(4):
+        for m in range(32):
+            banks = {(a_word_off(64, 16 * wq + (lane >> 2) + 8 * (m & 1), 4 * (m >> 1) + (lane & 3)) // 4) % 32 for lane in range(32)}
             assert len(banks) == 32
 
 

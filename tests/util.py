@@ -10,9 +10,61 @@ from keypointnerf_b200 import synthetic as syn
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
+# Golden files stay below 1 MB each: float32 arrays are stored losslessly as their four byte planes ("<key>__bp"; "<key>__bpd"
+# when the array is sorted along its last axis and its bit patterns are delta-coded along it first), which compresses far
+# better than the raw floats, and a fixture that is still too large is split into parts <name>.npz, <name>.1.npz, ...
+PART_BYTES = 900_000
+
+
+def _encode(k, a):
+    if a.dtype != np.float32 or a.ndim == 0:
+        return {k: a}
+    u = a.view(np.uint32)
+    suffix = "__bp"
+    if a.shape[-1] > 1 and bool(np.all(np.diff(a, axis=-1) >= 0)):
+        u = np.diff(u.astype(np.int64), axis=-1, prepend=0).astype(np.uint32)
+        suffix = "__bpd"
+    return {k + suffix: np.ascontiguousarray(np.moveaxis(u.view(np.uint8).reshape(u.shape + (4,)), -1, 0))}
+
+
+def _decode(k, a):
+    if k.endswith("__bpd") or k.endswith("__bp"):
+        u = np.ascontiguousarray(np.moveaxis(a, 0, -1)).view(np.uint32)[..., 0]
+        if k.endswith("__bpd"):
+            u = np.cumsum(u.astype(np.uint64), axis=-1).astype(np.uint32)
+        return k.rsplit("__", 1)[0], u.view(np.float32)
+    return k, a
+
+
+def save_golden(name, arrays, directory=GOLDEN):
+    import io
+    enc = {}
+    for k, a in arrays.items():
+        enc.update(_encode(k, np.asarray(a)))
+    parts, cur = [], {}
+    for k in sorted(enc, key=lambda k: enc[k].nbytes):
+        trial = dict(cur, **{k: enc[k]})
+        buf = io.BytesIO()
+        np.savez_compressed(buf, **trial)
+        if cur and len(buf.getvalue()) > PART_BYTES:
+            parts.append(cur)
+            cur = {k: enc[k]}
+        else:
+            cur = trial
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(os.path.join(directory, name + (f".{i}" if i else "") + ".npz"), **part)
+
+
 def load_golden(name):
-    z = np.load(os.path.join(GOLDEN, name + ".npz"))
-    g = {k: z[k] for k in z.files}
+    g, i = {}, 0
+    while True:
+        path = os.path.join(GOLDEN, name + (f".{i}" if i else "") + ".npz")
+        if not os.path.exists(path):
+            break
+        z = np.load(path)
+        g.update(_decode(k, z[k]) for k in z.files)
+        i += 1
     meta = json.loads(bytes(g.pop("meta")).decode())
     sha = bytes(g.pop("input_sha256")).decode()
     return g, meta, sha
