@@ -43,26 +43,33 @@ def look_at_extrinsic(azimuth: float, radius: float = 3.0, height: float = 0.0) 
     return Rt.astype(F32)
 
 
-def intrinsic(size: int, focal_at_512: float = 550.0) -> np.ndarray:
+def intrinsic(size: int, focal_at_512: float = 550.0, height: int | None = None) -> np.ndarray:
+    """Pinhole K for a ``size`` (width) x ``height`` image (square when ``height`` is None): the focal length scales with the
+    width, the principal point is the image centre (W/2, H/2)."""
+    height = size if height is None else height
     s = size / 512.0
     K = np.eye(4, dtype=np.float64)
     K[0, 0] = K[1, 1] = focal_at_512 * s
-    K[0, 2] = K[1, 2] = 256.0 * s
+    K[0, 2] = 256.0 * s
+    K[1, 2] = 256.0 * (height / 512.0)
     return K.astype(F32)
 
 
-def feature_shapes(src_size: int, n_views: int = 3):
-    """Shapes the reference encoders produce for ``src_size``^2 inputs (SURVEY.md section 8 header)."""
+def feature_shapes(src_size: int, n_views: int = 3, src_height: int | None = None):
+    """Shapes the reference encoders produce for ``src_size`` (width) x ``src_height`` inputs (square when ``src_height`` is
+    None; SURVEY.md section 8 header)."""
+    W, H = src_size, (src_size if src_height is None else src_height)
     return {
-        "feat64": (n_views, 64, src_size // 8, src_size // 8),
-        "feat8": (n_views, 8, src_size // 2, src_size // 2),
-        "feat_tex": (n_views, 8, src_size // 4, src_size // 4),
-        "img": (n_views, 3, src_size, src_size),
-        "fg": (n_views, 1, src_size, src_size),
+        "feat64": (n_views, 64, H // 8, W // 8),
+        "feat8": (n_views, 8, H // 2, W // 2),
+        "feat_tex": (n_views, 8, H // 4, W // 4),
+        "img": (n_views, 3, H, W),
+        "fg": (n_views, 1, H, W),
     }
 
 
-def silhouette_masks(K: np.ndarray, extrin: np.ndarray, src_size: int, semi_axes=(0.22, 0.64, 0.15)) -> np.ndarray:
+def silhouette_masks(K: np.ndarray, extrin: np.ndarray, src_size: int, semi_axes=(0.22, 0.64, 0.15),
+                     src_height: int | None = None) -> np.ndarray:
     """Foreground masks (V,1,H,W) bool = silhouettes of an origin-centred ellipsoid seen by each source camera.
 
     The intersection of the silhouette cones (the visual hull the validity test carves, reference ``src/model.py:729-739``)
@@ -70,10 +77,11 @@ def silhouette_masks(K: np.ndarray, extrin: np.ndarray, src_size: int, semi_axes
     rays that miss the box) is invalid: the reference's final-sample step (``dist[-1] = 1e10``, ``src/model.py:1166``) then
     multiplies a density of exactly 0 and no ray sits on that discontinuity (SURVEY.md section 7.4)."""
     V = K.shape[0]
-    ys, xs = np.meshgrid(np.arange(src_size, dtype=np.float64), np.arange(src_size, dtype=np.float64), indexing="ij")
+    W, H = src_size, (src_size if src_height is None else src_height)
+    ys, xs = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
     pix = np.stack([xs, ys, np.ones_like(xs)], -1).reshape(-1, 3)
     inv_ax = 1.0 / np.asarray(semi_axes, dtype=np.float64)
-    out = np.zeros((V, 1, src_size, src_size), dtype=bool)
+    out = np.zeros((V, 1, H, W), dtype=bool)
     for v in range(V):
         R = extrin[v, :3, :3].astype(np.float64)
         t = extrin[v, :3, 3].astype(np.float64)
@@ -83,14 +91,16 @@ def silhouette_masks(K: np.ndarray, extrin: np.ndarray, src_size: int, semi_axes
         a = (ds * ds).sum(-1)
         b = ds @ cs
         disc = b * b - a * ((cs * cs).sum() - 1.0)
-        out[v, 0] = (disc >= 0.0).reshape(src_size, src_size)
+        out[v, 0] = (disc >= 0.0).reshape(H, W)
     return out
 
 
 def make_scene(src_size: int = 512, n_views: int = 3, n_kpt: int = 18, seed: int = 2,
-               src_azimuths=(0.0, 2.1, 4.2), fg_hole: bool = False, fg_mode: str | None = None) -> dict:
+               src_azimuths=(0.0, 2.1, 4.2), fg_hole: bool = False, fg_mode: str | None = None,
+               src_height: int | None = None) -> dict:
     """Source-side inputs of the hot path (everything ``query`` reads, reference ``src/model.py:690-782``).
 
+    The source images are ``src_size`` wide and ``src_height`` high (square when ``src_height`` is None).
     ``fg_mode``: "ones" (SURVEY.md section 8d recipe, the bench scene) or "hull" (ellipsoid silhouettes, see
     ``silhouette_masks``); ``fg_hole`` additionally punches rectangular holes into either."""
     if fg_mode is None:
@@ -103,22 +113,23 @@ def make_scene(src_size: int = 512, n_views: int = 3, n_kpt: int = 18, seed: int
     bounds = np.stack([kpt3d[0].min(0) - 0.1, kpt3d[0].max(0) + 0.1], 0).astype(F32)[None]  # (1,2,3)
 
     rng = np.random.default_rng(seed)
-    sh = feature_shapes(src_size, n_views)
+    W, H = src_size, (src_size if src_height is None else src_height)
+    sh = feature_shapes(W, n_views, H)
     feat64 = rng.standard_normal(sh["feat64"], dtype=F32)
     feat8 = rng.standard_normal(sh["feat8"], dtype=F32)
     feat_tex = rng.standard_normal(sh["feat_tex"], dtype=F32)
     img = rng.random(sh["img"], dtype=F32)
-    K = intrinsic(src_size)
+    K = intrinsic(W, height=H)
     extrin = np.stack([look_at_extrinsic(a) for a in src_azimuths[:n_views]], 0)
     Ks = np.broadcast_to(K, (n_views, 4, 4)).copy()
-    fg = silhouette_masks(Ks, extrin, src_size) if fg_mode == "hull" else np.ones(sh["fg"], dtype=bool)
+    fg = silhouette_masks(Ks, extrin, W, src_height=H) if fg_mode == "hull" else np.ones(sh["fg"], dtype=bool)
     if fg_hole:
         # punch rectangular holes so that the foreground-mask term of the validity test
         # (reference src/model.py:737-739) is exercised, including its bilinear edge.
         for v in range(n_views):
-            a = src_size // 4 + v * (src_size // 16)
-            fg[v, 0, a:a + src_size // 8, a:a + src_size // 6] = False
-        fg[:, :, : src_size // 10, :] = False
+            ay, ax = H // 4 + v * (H // 16), W // 4 + v * (W // 16)
+            fg[v, 0, ay:ay + H // 8, ax:ax + W // 6] = False
+        fg[:, :, : H // 10, :] = False
 
     KRT = np.einsum("vij,vjk->vik", Ks.astype(np.float64), extrin.astype(np.float64)).astype(F32)
     return {
@@ -126,18 +137,21 @@ def make_scene(src_size: int = 512, n_views: int = 3, n_kpt: int = 18, seed: int
         "kpt3d": kpt3d, "bounds": bounds,
         "feat64": feat64, "feat8": feat8, "feat_tex": feat_tex, "img": img, "fg": fg,
         "K": Ks, "extrin": extrin, "KRT": KRT,
-        "width": float(src_size), "height": float(src_size),
+        "width": float(W), "height": float(H),
         "znear": 2.0, "zfar": 5.0, "nml_scale": 100.0,
     }
 
 
-def make_target(size: int = 512, azimuth: float = 1.0, znear: float = 2.0, zfar: float = 5.0, zoom: float = 1.0) -> dict:
+def make_target(size: int = 512, azimuth: float = 1.0, znear: float = 2.0, zfar: float = 5.0, zoom: float = 1.0,
+                width: int | None = None, height: int | None = None) -> dict:
     """Target camera dict as ``decode_batch`` builds it (reference ``src/model.py:309-414``); ``zoom`` scales the focal length
-    (small test targets zoom in so that most of their rays cross the visual hull)."""
-    K = intrinsic(size, 550.0 * zoom)[None]
+    (small test targets zoom in so that most of their rays cross the visual hull).  The image is ``width`` x ``height``
+    (each defaults to ``size``)."""
+    W, H = (size if width is None else width), (size if height is None else height)
+    K = intrinsic(W, 550.0 * zoom, height=H)[None]
     RT = look_at_extrinsic(azimuth)[None]
     KRT = (K[0].astype(np.float64) @ RT[0].astype(np.float64)).astype(F32)[None]
-    return {"K": K, "RT": RT, "KRT": KRT, "width": size, "height": size,
+    return {"K": K, "RT": RT, "KRT": KRT, "width": W, "height": H,
             "znear": znear, "zfar": zfar, "nml_scale": 100.0}
 
 

@@ -1,9 +1,14 @@
 """CPU oracle for the KeypointNeRF ray-march hot path.  TEST INFRASTRUCTURE ONLY.
 
-This file is a from-scratch restatement (plain fp32 torch-CPU tensor arithmetic, no
+This file is a from-scratch restatement (plain torch-CPU tensor arithmetic, no
 ``grid_sample``/``nn.Module``) of the algorithm the reference implements in
 ``/root/reference/src/model.py:690-1302``, ``src/spatial.py:63-118`` and
 ``src/utils.py:74-95,476-748``.  Each function cites the lines it follows.
+
+Precision: fp32 by default, like the reference.  ``with precision(torch.float64): ...`` runs the
+same arithmetic in fp64 (inputs, constants and intermediates), which gives a reference whose own
+round-off is far below any kernel's, so that a kernel's error can be told apart from the fp32
+oracle's.  The fp32 results do not depend on this switch existing.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline legs may
 import it; the product path (``keypointnerf_b200``) never does and has no CPU fallback.
@@ -15,6 +20,7 @@ container by ``tests/golden/make_golden.py`` and frozen under ``tests/golden/*.n
 """
 from __future__ import annotations
 
+import contextlib
 import math
 
 import numpy as np
@@ -22,8 +28,23 @@ import torch
 
 T = torch.Tensor
 
+_DTYPE = torch.float32   # arithmetic type of every function below (see ``precision``)
 
-def _t(x, dtype=torch.float32):
+
+@contextlib.contextmanager
+def precision(dtype: torch.dtype):
+    """Run the oracle in ``dtype`` (torch.float32 or torch.float64) inside the ``with`` block."""
+    global _DTYPE
+    assert dtype in (torch.float32, torch.float64)
+    prev, _DTYPE = _DTYPE, dtype
+    try:
+        yield
+    finally:
+        _DTYPE = prev
+
+
+def _t(x, dtype=None):
+    dtype = _DTYPE if dtype is None else dtype
     if isinstance(x, torch.Tensor):
         return x.to(dtype)
     return torch.as_tensor(np.asarray(x)).to(dtype)
@@ -73,11 +94,12 @@ def pixel_lattice(width: int, height: int, step: int, x_off: int, y_off: int) ->
     xs = torch.arange(0, width, step)
     yy, xx = torch.meshgrid(ys, xs, indexing="ij")
     g = torch.stack([xx + x_off, yy + y_off], -1).reshape(-1, 2)
-    return g.float()
+    return g.to(_DTYPE)
 
 
 def ray_setup(pix: T, K_t: T, RT_t: T, znear: float, zfar: float):
     """Rays through pixels (reference ``src/model.py:1026-1036``).  ``pix`` (R,2) float."""
+    pix = _t(pix)
     K3 = _t(K_t).reshape(-1, 4, 4)[0, :3, :3]
     RT = _t(RT_t).reshape(-1, 4, 4)[0]
     R, t = RT[:3, :3], RT[:3, 3]
@@ -94,7 +116,7 @@ def ray_setup(pix: T, K_t: T, RT_t: T, znear: float, zfar: float):
 
 def ray_bbox(bounds: T, o: T, d: T):
     """Slab test with the reference's "exactly two face hits" rule (``src/model.py:1178-1237``)."""
-    b = _t(bounds).reshape(2, 3) + torch.tensor([-0.01, 0.01])[:, None]
+    b = _t(bounds).reshape(2, 3) + torch.tensor([-0.01, 0.01], dtype=_DTYPE)[:, None]
     dd = d.clone()
     dd[dd.abs() < 1e-5] = 1e-5
     t6 = ((b[None] - o[:, None]) / dd[:, None]).reshape(-1, 6)  # order: min xyz, max xyz
@@ -119,7 +141,7 @@ def clip_near_far(n_r: T, f_r: T, near: T, far: T, hit: T):
 
 def coarse_z(n_r: T, f_r: T, S: int) -> T:
     """Uniform (eval, ``uniform=True``) depths (reference ``src/model.py:1045-1055``)."""
-    lin01 = torch.linspace(0.0, 1.0, steps=S)
+    lin01 = torch.linspace(0.0, 1.0, steps=S, dtype=_DTYPE)
     return n_r + (f_r - n_r) * lin01[None]
 
 
@@ -130,6 +152,7 @@ def project(scene: dict, pts: T):
     """World points -> normalised source-view coordinates (reference ``src/model.py:713-723``).
     Returns xy (V,N,2) in [-1,1] (align_corners convention) and z (V,N,1)."""
     KRT = _t(scene["KRT"])
+    pts = _t(pts)
     vh = torch.einsum("vij,nj->vni", KRT[:, :3, :3], pts) + KRT[:, None, :3, 3]
     zc = vh[..., 2:3]
     xy = vh[..., :2] / zc
@@ -185,7 +208,7 @@ def pixel_weight(xy: T, z: T, valid: T) -> T:
     xyz = 0.5 * torch.cat([xy, z], -1) + 0.5
     db = torch.minimum(xyz, 1.0 - xyz)
     s = torch.sigmoid(5.0 * (db / 0.1 - 1.0))
-    pw = (s[..., 0] * s[..., 1] * s[..., 2])[..., None] * valid[None, :, None].float()
+    pw = (s[..., 0] * s[..., 1] * s[..., 2])[..., None] * valid[None, :, None].to(s.dtype)
     return pw / (pw.sum(0, keepdim=True) + 1e-6)
 
 
@@ -195,12 +218,13 @@ def encode_rel_z_decay(scene: dict, pts: T, sp_level: int = 3, scale: float = 1.
     Output (V,N,(1+2L)K) with layout [r*K+k], r = 0: dz, 1+2l: sin(pi 2^l dz), 2+2l: cos(pi 2^l dz)."""
     E = _t(scene["extrin"])
     kpt = _t(scene["kpt3d"]).reshape(-1, 3)
+    pts = _t(pts)
     c = torch.einsum("vij,nj->vni", E[:, :3, :3], pts) + E[:, None, :3, 3]  # (V,N,3)
     ck = torch.einsum("vij,kj->vki", E[:, :3, :3], kpt) + E[:, None, :3, 3]  # (V,K,3)
     dz = scale * (c[:, :, None, 2] - ck[:, None, :, 2])  # (V,N,K)
     d2 = ((c[:, :, None, :] - ck[:, None, :, :]) ** 2).sum(-1)
     wk = torch.exp(-d2 / (2.0 * sigma ** 2))
-    freqs = [np.float32(np.pi * (2 ** l)) for l in range(sp_level)]
+    freqs = [np.float32(np.pi * (2 ** l)) if _DTYPE == torch.float32 else np.pi * (2 ** l) for l in range(sp_level)]
     y = torch.stack([dz * float(f) for f in freqs], 2)  # (V,N,L,K)
     # reference layout: cat(sin(y), cos(y)) along the keypoint axis then flattened:
     # [dz(K) | l0: sin(K) cos(K) | l1: sin cos | ...]  (src/spatial.py:35-39)
@@ -245,6 +269,7 @@ def source_centres(scene: dict) -> T:
 def ray_diff(scene: dict, pts: T, view: T) -> T:
     """[unit(dir - dir_src), dir . dir_src] per view (reference ``src/model.py:825-832``).  (V,N,4)"""
     C = source_centres(scene)
+    pts, view = _t(pts), _t(view)
     r = pts[None] - C[:, None]
     r = r / r.norm(dim=-1, keepdim=True).clamp_min(1e-12)
     diff = view[None] - r
@@ -286,6 +311,7 @@ def query(scene: dict, fw: dict, pts: T, view: T, sp: dict | None = None,
     """``KeypointNeRF.query`` + ``query_color`` (reference ``src/model.py:690-843``).
     pts, view (N,3).  Returns out (N,5) = [sdf_raw, rad, r, g, b] and valid (N,) bool."""
     sp = sp or {}
+    pts, view = _t(pts), _t(view)
     xy, z = project(scene, pts)
     valid = validity(scene, xy, z, disable_fg_mask)
     pw = pixel_weight(xy, z, valid)
@@ -302,7 +328,7 @@ def query(scene: dict, fw: dict, pts: T, view: T, sp: dict | None = None,
     V = xy.shape[0]
     f = torch.cat([rgb_src, tex, lat[None].expand(V, -1, -1)], -1)
     rd = ray_diff(scene, pts, view)
-    mask = valid[None, :, None].float().expand(V, -1, -1)
+    mask = valid[None, :, None].to(xy.dtype).expand(V, -1, -1)
     rgb = ibr_head(fw, f, rd, mask, rgb_src)
     out = torch.cat([geo, rgb], -1)
     if return_parts:
@@ -319,7 +345,7 @@ def eval_func(scene: dict, fw: dict, pts: T, view: T, sp=None, chunk: int = 1 <<
     outs = []
     for s in range(0, pts.shape[0], chunk):
         o, valid = query(scene, fw, pts[s:s + chunk], view[s:s + chunk], sp, disable_fg_mask)
-        m = valid.float()[:, None]
+        m = valid.to(o.dtype)[:, None]
         sdf = m * o[:, :1] + (1.0 - m) * (0.1 / float(scene["nml_scale"]))
         alpha = m * torch.relu(o[:, 1:2])
         outs.append(torch.cat([alpha, sdf, o[:, 2:]], -1))
@@ -349,7 +375,7 @@ def importance_sample(contrib_mid: T, z_mid: T, S_f: int) -> T:
     c = contrib_mid + 1e-5
     pdf = c / c.sum(-1, keepdim=True)
     cdf = torch.cat([torch.zeros_like(pdf[:, :1]), torch.cumsum(pdf, -1)], -1)
-    u = torch.linspace(0.0, 1.0, steps=S_f)[None].expand(cdf.shape[0], -1).contiguous()
+    u = torch.linspace(0.0, 1.0, steps=S_f, dtype=contrib_mid.dtype)[None].expand(cdf.shape[0], -1).contiguous()
     idx = torch.searchsorted(cdf.contiguous(), u, right=True)
     lo = (idx - 1).clamp(min=0)
     hi = idx.clamp(max=cdf.shape[-1] - 1)

@@ -190,6 +190,11 @@ CASES = {
                   capture="all"),
     "tiny_k24": _c(src_size=64, tgt_size=32, zoom=2.0, azimuth=2.5, level=1, S_c=12, S_f=8, fine=True, n_kpt=24,
                    scene_seed=3, w_seed=5, capture="all"),
+    # non-square sources (128 wide x 80 high) and targets (48 x 32): every width / height pair is read separately
+    "rect": _c(src_size=128, src_height=80, tgt_size=48, tgt_width=48, tgt_height=32, zoom=3.5, level=1, S_c=16, S_f=16,
+               fine=True, fg_hole=True, capture="all"),
+    "rect_k24": _c(src_size=128, src_height=80, tgt_size=48, tgt_width=48, tgt_height=32, zoom=3.0, azimuth=2.5, level=2,
+                   x_off=1, y_off=1, S_c=12, S_f=8, fine=True, n_kpt=24, scene_seed=3, w_seed=5, capture="all"),
     # BASELINE config 1: one 64x64 strided pass, 32 samples/ray, 512^2 sources (hull scene and the bench scene)
     "cfg1_tile": _c(),
     "cfg1_ones": _c(fg_mode="ones", capture="some"),
@@ -213,9 +218,10 @@ def main():
     for name in names:
         c = CASES[name]
         scene = syn.make_scene(src_size=c["src_size"], n_views=3, n_kpt=c["n_kpt"], seed=c["scene_seed"],
-                               fg_mode=c["fg_mode"], fg_hole=c["fg_hole"])
+                               fg_mode=c["fg_mode"], fg_hole=c["fg_hole"], src_height=c.get("src_height"))
         weights = syn.make_weights(c["n_kpt"], seed=c["w_seed"])
-        target = syn.make_target(size=c["tgt_size"], azimuth=c["azimuth"], zoom=c["zoom"])
+        target = syn.make_target(size=c["tgt_size"], azimuth=c["azimuth"], zoom=c["zoom"], width=c.get("tgt_width"),
+                                 height=c.get("tgt_height"))
         key = (c["n_kpt"], c["w_seed"])
         if key not in nets:
             nets[key] = build_net(M, c["n_kpt"], weights)

@@ -22,7 +22,7 @@ import torch
 from keypointnerf_b200 import synthetic as syn
 from keypointnerf_b200.testing import build_model, scene_tensors
 from oracle import kpnerf_oracle as O  # checker only
-from tests.util import checksum, load_golden, psnr, scene_from_meta
+from tests.util import checksum, load_golden, psnr, scene_from_meta, target_wh
 
 pytestmark = pytest.mark.gpu
 
@@ -70,15 +70,15 @@ def _render_tile(net, meta, scene, target, dev="cuda:0", engine=0, fine=None, de
     fine = meta["fine"] if fine is None else fine
     m = net._bind_scene(a["cam"], a["feat_geo"], a["feat_tex"], a["sp_data"], a["img"], a["fg"], a["bounds"])
     step = 2 ** (meta["level"] - 1)
-    n = meta["tgt_size"] // step
+    w, h = target_wh(meta)
     res = m.render(K=a["cam_tar"]["K"], RT=a["cam_tar"]["RT"], znear=target["znear"], zfar=target["zfar"],
-                   x0=meta["x_off"], y0=meta["y_off"], step=step, nx=n, ny=n, S_c=meta["S_c"], S_f=meta["S_f"],
+                   x0=meta["x_off"], y0=meta["y_off"], step=step, nx=w // step, ny=h // step, S_c=meta["S_c"], S_f=meta["S_f"],
                    fine=fine, engine=engine, debug=debug, z_fine_override=z_override)
     torch.cuda.synchronize()
     return {k: v.cpu().numpy() for k, v in res.items()}
 
 
-@pytest.fixture(scope="module", params=["tiny", "tiny_fg", "tiny_k24"])
+@pytest.fixture(scope="module", params=["tiny", "tiny_fg", "tiny_k24", "rect", "rect_k24"])
 def case(request):
     g, meta, sha = load_golden(request.param)
     scene, weights, target = scene_from_meta(meta)
@@ -259,6 +259,30 @@ def test_engines_agree_per_sample():
     d = (o0 - o1).abs()[v1]
     print(f"engines per-sample: rgb {float(d[:, 2:].max()):.2e} rad {float(d[:, 1].max()):.2e} sdf {float(d[:, 0].max()):.2e}")
     assert float(d[:, 2:].max()) < 5e-4 and float(d[:, 1].max()) < 5e-2 and float(d[:, 0].max()) < 5e-3
+
+
+def test_non_square_frame_through_the_model_api():
+    """The non-square fixture (128 x 80 sources, 48 x 32 target) through KeypointNeRF.batch_render_pifu_nerf: the images come
+    back (1, 3, 32, 48) / (1, 32, 48) like the reference's, and match the reference's own images, coarse and free-running fine."""
+    g, meta, scene, weights, target, net = _golden_case("rect")
+    a = scene_tensors(scene, target, "cuda:0")
+    net.engine = 0
+    with torch.no_grad():
+        o = net.batch_render_pifu_nerf(net, a["img"], a["cam"], 3, a["cam_tar"], meta["level"], torch.Tensor([[0, 0]]), None,
+                                       a["feat_geo"], a["feat_tex"], a["sp_data"], None, sample_per_ray_c=meta["S_c"],
+                                       sample_per_ray_f=meta["S_f"], fine=True, uniform=True, src_foreground_mask=a["fg"],
+                                       bounds=a["bounds"])
+    torch.cuda.synchronize()
+    assert o["tex_fg"].shape == (1, 3, 32, 48) and o["tex_fg_fine"].shape == (1, 3, 32, 48)
+    for k in ("depth", "alpha", "alpha_fine", "sdf"):
+        assert o[k].shape == (1, 32, 48), k
+    t = TOL[0]
+    rep = []
+    good = check(rep, "tex_fg", o["tex_fg"].cpu().numpy(), g["tex_fg"], ALL, t["rgb"])
+    good &= check(rep, "alpha", o["alpha"].cpu().numpy(), g["alpha"], ALL, t["alpha"])
+    p = psnr(o["tex_fg_fine"].cpu().numpy(), g["tex_fg_fine"])
+    print("rect through the model API: " + "; ".join(rep) + f"; fine psnr {p:.1f} dB")
+    assert good and p > 50.0, rep
 
 
 def test_api_shapes_and_host_path_equal_device_path():
@@ -568,17 +592,22 @@ def test_front_kernel_validity_is_exact():
     weights = syn.make_weights(18)
     net = build_model(weights, 18, "cuda:0")
     cases = [dict(fg_mode="ones", fg_hole=False, size=48, az=1.0, zoom=1.0), dict(fg_mode="hull", fg_hole=False, size=64, az=2.0, zoom=1.5),
-             dict(fg_mode="hull", fg_hole=True, size=40, az=0.3, zoom=3.0), dict(fg_mode="ones", fg_hole=True, size=56, az=4.4, zoom=0.6)]
+             dict(fg_mode="hull", fg_hole=True, size=40, az=0.3, zoom=3.0), dict(fg_mode="ones", fg_hole=True, size=56, az=4.4, zoom=0.6),
+             # non-square sources (128 x 80) and target (56 x 40), foreground masks at half the image resolution (64 x 40)
+             dict(fg_mode="hull", fg_hole=True, size=56, height=40, az=1.2, zoom=2.5, src_height=80, fg_half=True)]
     for c in cases:
-        scene = syn.make_scene(src_size=128, n_kpt=18, fg_mode=c["fg_mode"], fg_hole=c["fg_hole"])
-        target = syn.make_target(size=c["size"], azimuth=c["az"], zoom=c["zoom"])
+        scene = syn.make_scene(src_size=128, n_kpt=18, fg_mode=c["fg_mode"], fg_hole=c["fg_hole"], src_height=c.get("src_height"))
+        if c.get("fg_half"):
+            scene["fg"] = np.ascontiguousarray(scene["fg"][:, :, ::2, ::2])
+        nx, ny = c["size"], c.get("height", c["size"])
+        target = syn.make_target(size=c["size"], azimuth=c["az"], zoom=c["zoom"], width=nx, height=ny)
         a = scene_tensors(scene, target, "cuda:0")
         m = net._bind_scene(a["cam"], a["feat_geo"], a["feat_tex"], a["sp_data"], a["img"], a["fg"], a["bounds"])
-        n, S_c, S_f = c["size"], 24, 16
-        r = m.render(K=a["cam_tar"]["K"], RT=a["cam_tar"]["RT"], znear=2.0, zfar=5.0, x0=0, y0=0, step=1, nx=n, ny=n, S_c=S_c, S_f=S_f,
+        S_c, S_f = 24, 16
+        r = m.render(K=a["cam_tar"]["K"], RT=a["cam_tar"]["RT"], znear=2.0, zfar=5.0, x0=0, y0=0, step=1, nx=nx, ny=ny, S_c=S_c, S_f=S_f,
                      fine=True, engine=1, debug=True)
         got = m.stats()["samples_valid"]
-        pix = O.pixel_lattice(n, n, 1, 0, 0)
+        pix = O.pixel_lattice(nx, ny, 1, 0, 0)
         o, d, n_r, f_r = O.ray_setup(pix, target["K"], target["RT"], 2.0, 5.0)
         near, far, hit = O.ray_bbox(scene["bounds"], o, d)
         n_r, f_r = O.clip_near_far(n_r, f_r, near, far, hit)

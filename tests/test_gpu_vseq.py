@@ -12,7 +12,7 @@ from tests.util import psnr
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("name", ["tiny", "tiny_fg", "cfg1_tile", "cfg2_pass", "cfg4_pass"])
+@pytest.mark.parametrize("name", ["tiny", "tiny_fg", "rect", "rect_k24", "cfg1_tile", "cfg2_pass", "cfg4_pass"])
 def test_vseq_matches_reference(name):
     g, meta, scene, weights, target, net = _golden_case(name)
     r = _render_tile(net, dict(meta, fine=False), scene, target, engine=3)

@@ -12,7 +12,7 @@ from oracle import kpnerf_oracle as O
 from tests.util import checksum, load_golden, scene_from_meta, psnr
 
 
-@pytest.fixture(scope="module", params=["tiny", "tiny_fg", "tiny_k24"])
+@pytest.fixture(scope="module", params=["tiny", "tiny_fg", "tiny_k24", "rect", "rect_k24"])
 def case(request):
     g, meta, sha = load_golden(request.param)
     scene, weights, target = scene_from_meta(meta)
@@ -21,6 +21,31 @@ def case(request):
 
 
 def test_query_stages_match_reference(case):
+    check_query_stages(case)
+
+
+def test_tile_coarse_matches_reference(case):
+    check_tile_coarse(case)
+
+
+def test_tile_fine_matches_reference(case):
+    check_tile_fine(case)
+
+
+def test_fp64_oracle_meets_the_same_tolerances(case):
+    """The oracle run in fp64 (the high-precision yardstick of the GPU tests) is the same algorithm as the reference: it meets
+    every tolerance the fp32 oracle is held to, on every stage.  One exception: the samples of the half-resolution map f8 differ
+    from the reference's by up to 1.9e-5 (rect_k24; 1.0e-5 on the square cases), against 1e-5 for the fp32 oracle.  That is the
+    reference's own fp32 round-off of the projected coordinates, times the texel-to-texel slope of a random map with W/2 texels;
+    the fp32 oracle makes the same rounding and so agrees with it more closely."""
+    with O.precision(torch.float64):
+        assert O.fold_weights(case[3])["ani_al"].dtype == torch.float64
+        check_query_stages(case, f8_atol=3e-5)
+        check_tile_coarse(case)
+        check_tile_fine(case)
+
+
+def check_query_stages(case, f8_atol=1e-5):
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
     pts = torch.from_numpy(g["query_pts"])
@@ -30,7 +55,7 @@ def test_query_stages_match_reference(case):
     assert np.array_equal(valid.numpy(), g["query_valid"])
     np.testing.assert_allclose(parts["pw"][..., 0].numpy(), g["pw"], atol=2e-6)
     np.testing.assert_allclose(parts["f64"].numpy()[:, sel], g["f64"], atol=1e-5)
-    np.testing.assert_allclose(parts["f8"].numpy()[:, sel], g["f8"], atol=1e-5)
+    np.testing.assert_allclose(parts["f8"].numpy()[:, sel], g["f8"], atol=f8_atol)
     np.testing.assert_allclose(parts["enc"].numpy()[:, sel], g["enc"], atol=2e-5)
     np.testing.assert_allclose(parts["x_view"].numpy()[:, sel], g["x_view"], atol=1e-4)
     np.testing.assert_allclose(parts["x_pool"].numpy()[sel], g["x_pool"], atol=1e-4)
@@ -43,7 +68,7 @@ def test_query_stages_match_reference(case):
     np.testing.assert_allclose(out.numpy()[v], g["query_out"][v], atol=2e-3, rtol=1e-4)
 
 
-def test_tile_coarse_matches_reference(case):
+def check_tile_coarse(case):
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
     r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True)
@@ -55,7 +80,7 @@ def test_tile_coarse_matches_reference(case):
     np.testing.assert_allclose(r["depth"].numpy(), g["depth"][0], atol=2e-4)
 
 
-def test_tile_fine_matches_reference(case):
+def check_tile_fine(case):
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
     r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True)

@@ -19,7 +19,7 @@ PART_BYTES = 900_000
 def _encode(k, a):
     if a.dtype != np.float32 or a.ndim == 0:
         return {k: a}
-    u = a.view(np.uint32)
+    u = np.ascontiguousarray(a).view(np.uint32)
     suffix = "__bp"
     if a.shape[-1] > 1 and bool(np.all(np.diff(a, axis=-1) >= 0)):
         u = np.diff(u.astype(np.int64), axis=-1, prepend=0).astype(np.uint32)
@@ -70,11 +70,19 @@ def load_golden(name):
     return g, meta, sha
 
 
+def target_wh(meta):
+    """(width, height) of a fixture's target image; fixtures without the keys are square."""
+    return int(meta.get("tgt_width") or meta["tgt_size"]), int(meta.get("tgt_height") or meta["tgt_size"])
+
+
 def scene_from_meta(meta):
+    """Seeded scene, weights and target of a fixture.  ``src_height`` / ``tgt_width`` / ``tgt_height`` describe non-square
+    sources and targets; older fixtures do not have them and are square (``src_size`` / ``tgt_size``)."""
     scene = syn.make_scene(src_size=meta["src_size"], n_views=3, n_kpt=meta["n_kpt"], seed=meta["scene_seed"],
-                           fg_hole=meta["fg_hole"], fg_mode=meta.get("fg_mode", "ones"))
+                           fg_hole=meta["fg_hole"], fg_mode=meta.get("fg_mode", "ones"), src_height=meta.get("src_height"))
     weights = syn.make_weights(meta["n_kpt"], seed=meta["w_seed"])
-    target = syn.make_target(size=meta["tgt_size"], azimuth=meta["azimuth"], zoom=meta.get("zoom", 1.0))
+    w, h = target_wh(meta)
+    target = syn.make_target(size=meta["tgt_size"], azimuth=meta["azimuth"], zoom=meta.get("zoom", 1.0), width=w, height=h)
     return scene, weights, target
 
 
