@@ -121,8 +121,9 @@ typedef struct {
   int engine;             /* 0 = default: tensor cores (wgmma), fp16 operands, fp32 accumulate; the density tail (stages P0|compress,
                                  P1) runs with two-term (hi+lo) weights and activations;
                              1 = fp32 CUDA-core engine (parity anchor, ~25x slower; the ONLY engine for shapes the tensor-core
-                                 engine does not cover: n_views != 3, n_kpt not in {18,24}, sp_level != 3 -- such shapes
-                                 fail with KPN_ERR_UNSUPPORTED unless engine = 1 is requested explicitly);
+                                 engine does not cover: n_views != 3, sp_level != 3 -- such shapes fail with
+                                 KPN_ERR_UNSUPPORTED unless engine = 1 is requested explicitly).  Every engine takes any
+                                 1 <= n_kpt <= KPN_MAX_KPT;
                              2 = as 0 with single-term fp16 weights in the density tail (more rounding error);
                              3, 4 = as 0 (they selected between two geometry kernels of an earlier architecture; one kernel
                                  serves both here) */
@@ -210,8 +211,9 @@ int kpn_decode_views(kpn_ctx* ctx, const uint8_t* images, const uint8_t* masks, 
  * flag afterwards.  kpn_get_stats reports a raised flag as KPN_ERR_CUDA.  Synchronises the device. */
 int kpn_debug_timing(kpn_ctx* ctx, int enable, unsigned long long* out16);
 
-/* Host-only test hook (no GPU needed): tensor-core engine's input permutation of geometry stage `stage` (0..5) for n_kpt in
- * {18, 24}: kmap_out[i] = K index input i is multiplied with, *kbias_out = K index of the bias row, *kpad_out = padded K. */
+/* Host-only test hook (no GPU needed): tensor-core engine's input permutation of geometry stage `stage` (0..5) for
+ * 1 <= n_kpt <= KPN_MAX_KPT: kmap_out[i] = K index input i is multiplied with, *kbias_out = K index of the bias row,
+ * *kpad_out = padded K.  n_inputs must be the stage's input count (stage 0: 7 n_kpt + 64; 1..5: 128, 136, 120, 128, 64). */
 int kpn_debug_kmap(int stage, int n_kpt, int n_inputs, int* kmap_out, int* kbias_out, int* kpad_out);
 
 /* Debug hook kept for ABI stability: per-stage cycle stamps of an instrumented build; no instrumented build of the

@@ -191,7 +191,7 @@ extern "C" int kpn_set_weights(kpn_ctx* c, const kpn_weights* w) {
   DeviceGuard g(c->device);
   if (w->n_kpt < 1 || w->n_kpt > simt_max_kpt() || w->n_kpt > KPN_MAX_KPT)
     KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "n_kpt=%d unsupported (1..%d)", w->n_kpt, simt_max_kpt());
-  if (w->sp_level < 0 || w->sp_level > MAX_SPL || (1 + 2 * w->sp_level) * w->n_kpt + 64 > 232)
+  if (w->sp_level < 0 || w->sp_level > MAX_SPL || (1 + 2 * w->sp_level) * w->n_kpt + 64 > simt_max_geo_input())
     KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "sp_level=%d unsupported", w->sp_level);
   int dims[NLAYER][2];
   expected_dims(w->n_kpt, w->sp_level, dims);
@@ -381,9 +381,9 @@ static int shade_batch(kpn_ctx* c, const SampleSrc& src, const int* list, const 
   const bool use_tc = engine != 1;
   if (engine < 0 || engine > 4) KPN_FAIL(c, KPN_ERR_ARG, "kpn_opts.engine = %d (0 .. 4)", engine);
   if (use_tc && !(c->tc_weights && tc_supported(c->scene_views, c->n_kpt, c->sp_level)))
-    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "the tensor-core engine covers n_views == 3, n_kpt in {18, 24}, sp_level == 3; this scene has "
+    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "the tensor-core engine covers n_views == 3, 1 <= n_kpt <= %d, sp_level == 3; this scene has "
              "n_views=%d n_kpt=%d sp_level=%d: request engine = 1 (fp32 CUDA-core engine, ~25x slower) explicitly",
-             c->scene_views, c->n_kpt, c->sp_level);
+             KPN_MAX_KPT, c->scene_views, c->n_kpt, c->sp_level);
   cudaEvent_t e0 = nullptr, em = nullptr, e1 = nullptr;   // start | after the geometry kernel | stop
   if (c->profiling) {
     while (c->ev_used + 3 > c->ev_pool.size()) {
@@ -699,9 +699,14 @@ extern "C" int kpn_debug_timing(kpn_ctx* c, int enable, unsigned long long* out1
 }
 
 // Host-only test hook: the K index (element of the fp16 activation row) each input of a geometry stage is multiplied with, and
-// the K index of its bias row (tests/test_host_abi.py checks that the layer-0 permutation is a bijection).
+// the K index of its bias row, for every keypoint count the tensor-core engine covers (tests/test_host_abi.py and
+// tests/test_kpt_layout_cpu.py check that the layer-0 permutation is a bijection).
+// n_inputs must be the stage's input count (the map is a permutation of exactly those inputs; an index past them has no K row).
 extern "C" int kpn_debug_kmap(int stage, int n_kpt, int n_inputs, int* kmap_out, int* kbias_out, int* kpad_out) {
-  if (stage < 0 || stage > 5 || !tc_supported(3, n_kpt, 3) || n_inputs < 0 || !kmap_out) return KPN_ERR_ARG;
+  if (stage < 0 || stage > 5 || !tc_supported(3, n_kpt, 3) || !kmap_out) return KPN_ERR_ARG;
+  int dims[NLAYER][2];
+  expected_dims(n_kpt, 3, dims);   // geometry stages 0..5 are layers 0..5 (stage 4 also stacks the compress layer, same input)
+  if (n_inputs != dims[stage][1]) return KPN_ERR_ARG;
   for (int i = 0; i < n_inputs; ++i) kmap_out[i] = tc_kmap(stage, n_kpt, i);
   if (kbias_out) *kbias_out = tc_kbias(stage, n_kpt);
   if (kpad_out) *kpad_out = make_tc_plan(n_kpt).st[stage].Kp;

@@ -408,7 +408,8 @@ __global__ void compact_kernel(const DevScene* __restrict__ sc, SampleSrc src, l
 // ------------------------------------------------------------------------------------------------
 constexpr int TS = 64;
 constexpr int NT = 256;
-constexpr int LDA = 232;  // 7*MAXK(=24 supported here)+64, multiple of 4
+constexpr int LDA = 7 * MAXK + 64;  // widest geometry input (7*KPN_MAX_KPT encodings + feat64) = 288 floats, multiple of 4
+static_assert(LDA % 4 == 0, "rows are read as float4");
 constexpr int LDB = 128;
 
 enum { ACT_NONE = 0, ACT_SP = 1, ACT_ELU = 2 };
@@ -1001,5 +1002,6 @@ cudaError_t launch_resample(const int* list, const float* cw, const int* start0,
 }
 int max_coarse_samples() { return MAX_SC; }
 int simt_max_kpt() { return (LDA - 64) / 7; }
+int simt_max_geo_input() { return LDA; }
 
 }  // namespace kpn

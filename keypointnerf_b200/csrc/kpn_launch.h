@@ -44,5 +44,6 @@ cudaError_t launch_decode_views(const uint8_t* images, const uint8_t* masks, con
                                 float* out_img, uint8_t* out_mask, cudaStream_t st);
 int max_coarse_samples();
 int simt_max_kpt();
+int simt_max_geo_input();   // widest geometry-layer-0 input ((1 + 2 sp_level) n_kpt + 64) the fp32 engine's tile rows hold
 
 }  // namespace kpn

@@ -20,9 +20,11 @@
 // Stage table:
 //   geo    0 L0 190->128 | 1 L1 128->128 | 2 L2 136->120 | 3 L3 120->64 | 4 P0|CMP 128->64|24 | 5 P1 64->64
 //   colour 12 RE1 16->35 | 6 BASE0 105->64 | 7 BASE1 64->32 | 8 VIS1A 32->32 | 9 VIS1B 32->33 | 10 VIS2A 32->32 | 11 OUT0 37->16
+#include <array>
 #include <atomic>
 #include <cstdlib>
 #include <type_traits>
+#include <utility>
 #include "kpn_device.cuh"
 #include "kpn_launch.h"
 #include "kpn_tc.cuh"
@@ -235,13 +237,31 @@ struct Group {   // the 3-view group of this lane: the other two lanes
 // column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
 // pooling columns, as tc_kmap's runs are laid out).  20 samples per tile.
 // =====================================================================================================================
-constexpr int GWG = 2;                        // warpgroups per CTA (front and tail kernels)
+constexpr int GWG = 2;                        // warpgroups per CTA (tail kernel; front kernel up to 28 keypoints)
 constexpr int FSPT = 2 * SPW;                 // samples per front tile
 constexpr int D3S = 68;                       // row stride (floats) of the L3 accumulator rows staged for the pooling
 constexpr int POOL_W = 128;                   // pooled [mean 64 | var 64] fp32 per sample
 constexpr long long POOL_SLICE = 1ll << 22;   // samples per front/tail launch pair (bounds the pooled scratch to 2 GiB)
-__host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) { return 64u * (uint32_t)tc_k0p(n_kpt) * 2u; }
-static_assert(64 * D3S * 4 <= 64 * 192 * 2, "the L3 rows fit in the activation tile they replace");
+// activation tile of a front warpgroup: 64 rows of the layer-0 input, which is at least as wide as the 144-wide inputs of
+// L1 / L2 for 9 keypoints and more; fewer keypoints get the L1 / L2 width
+__host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) {
+  return 64u * (uint32_t)(tc_k0p(n_kpt) > 144 ? tc_k0p(n_kpt) : 144) * 2u;
+}
+static_assert(64 * D3S * 4 <= 64 * 144 * 2, "the L3 rows fit in the activation tile they replace");
+// Warpgroups per front CTA: two while the resident W_hi of stages 0..3 and two activation tiles fit in the 227 KB an SM
+// gives a block (up to 28 keypoints: 229 376 B dynamic + the static scene block), one above (29..32 keypoints: K0P 288 / 304)
+constexpr uint32_t SMEM_OPTIN = 227u * 1024u;
+constexpr uint32_t FRONT_STATIC = 2048u;      // static shared memory of the front kernel (SceneS + mbarrier, ptxas)
+static_assert(sizeof(SceneS) + sizeof(uint64_t) <= FRONT_STATIC, "static shared memory of the front kernel");
+__host__ __device__ constexpr uint32_t front_smem_bytes(int n_kpt, int wgs) {
+  return make_tc_plan(n_kpt).st[4].off + (uint32_t)wgs * front_tile_bytes(n_kpt);
+}
+__host__ __device__ constexpr int front_wgs(int n_kpt) { return front_smem_bytes(n_kpt, 2) + FRONT_STATIC <= SMEM_OPTIN ? 2 : 1; }
+static_assert(front_wgs(18) == 2 && front_wgs(24) == 2 && front_wgs(28) == 2 && front_wgs(29) == 1, "front CTA layouts");
+static_assert(front_smem_bytes(KPN_MAX_KPT, 1) + FRONT_STATIC <= SMEM_OPTIN, "one warpgroup fits at the maximum count");
+// offsets of the tail's (4, 5) and the colour head's (6..12) tiles relative to the first of them; the tiles past stage 0 have
+// the same size for every keypoint count, so any count's plan gives them
+constexpr TcPlan REL_PLAN = make_tc_plan(KPN_MAX_KPT);
 
 // one geometry stage of the warpgroup: A (64 rows at `a`) x resident W tile at `b` -> d (N = 128 or 64 fp32 per row)
 template <int N, int KCH>
@@ -265,21 +285,39 @@ __device__ __forceinline__ void front_epi_sp(const float* d, uint8_t* a, int wq,
   }
 }
 
-template <int NK>
-__global__ void __launch_bounds__(GWG * 128, 1)
-geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ wblob, SampleSrc src, const int* __restrict__ list,
-                 const int* __restrict__ count_ptr, long long base, long long len, float* __restrict__ pool) {
+// keypoint encodings of pair j (keypoints 2j, 2j+1) as 7 packed fp16 words; the second slot of an odd count's last pair is 0
+template <int NP>
+__device__ __forceinline__ void encode_pair(const SceneS& S, int v, int j, int nk, const float c[3], uint32_t* a) {
+  float e0[7], e1[7];
+  encode_fast(S, v, 2 * j, c, e0);
+  if (j < NP - 1 || 2 * j + 1 < nk) {
+    encode_fast(S, v, 2 * j + 1, c, e1);
+  } else {
+#pragma unroll
+    for (int r = 0; r < 7; ++r) e1[r] = 0.0f;
+  }
+#pragma unroll
+  for (int r = 0; r < 7; ++r) a[r] = tc::pack_h2(e0[r], e1[r]);
+}
+
+// One instantiation per keypoint pair count NP (nk = 2 NP - 1 or 2 NP keypoints).
+template <int NP>
+__global__ void __launch_bounds__(front_wgs(2 * NP) * 128, 1)
+geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __restrict__ wblob, SampleSrc src,
+                 const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
+                 float* __restrict__ pool) {
   extern __shared__ __align__(1024) uint8_t wsm[];
   __shared__ uint64_t wbar;
   __shared__ SceneS scs;
+  constexpr int NK = 2 * NP, FWG = front_wgs(NK);
   constexpr TcPlan plan = make_tc_plan(NK);
   constexpr uint32_t WBYTES = plan.st[4].off;        // W_hi of stages 0..3
-  constexpr int NP = NK / 2, PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
+  constexpr int PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
   const long long end = min((long long)*count_ptr, base + len);
   if (end <= base) return;
   const int ntiles = (int)((end - base + FSPT - 1) / FSPT);
   const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31;
-  stage_scene(scs, *scp, NK, t, GWG * 128);
+  stage_scene(scs, *scp, nk, t, FWG * 128);
   if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
   __syncthreads();
   if (t == 0) load_weights(wsm, wblob, WBYTES, &wbar);
@@ -291,7 +329,7 @@ geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ w
   const int row = (wq & 1) * 32 + lane, h = wq >> 1;
   const int g = lane / 3, v = lane - 3 * g;           // lanes 30, 31 replay views 0, 1 of the warp's last sample (unused)
   const Group grp(lane);
-  for (int tile = blockIdx.x * GWG + wg; tile < ntiles; tile += gridDim.x * GWG) {
+  for (int tile = blockIdx.x * FWG + wg; tile < ntiles; tile += gridDim.x * FWG) {
     const long long si = base + (long long)tile * FSPT + (wq & 1) * SPW + min(g, SPW - 1);
     const int id = list[min(si, end - 1)];
     float p[3], dd[3];
@@ -307,9 +345,10 @@ geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ w
       c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
       c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
       const Taps t64 = make_taps(q.u, q.v, scs.f64.W, scs.f64.H);
+      constexpr int C1 = 7 * PA + FA / 2;             // thread 0's run: words [0, C1); thread 1's: [C1, K0P / 2)
+      static_assert(C1 % 4 == 0 && C1 > 0, "both runs start on a 16-byte chunk");
       if (h == 0) {
-        constexpr int N0 = 7 * PA + FA / 2;
-        uint32_t a[N0];
+        uint32_t a[C1];
 #pragma unroll
         for (int gq = 0; gq < FA / 4; ++gq) {
           float f[4];
@@ -318,18 +357,12 @@ geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ w
           a[7 * PA + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
         }
 #pragma unroll
-        for (int j = 0; j < PA; ++j) {
-          float e0[7], e1[7];
-          encode_fast(scs, v, 2 * j, c, e0);
-          encode_fast(scs, v, 2 * j + 1, c, e1);
-#pragma unroll
-          for (int r = 0; r < 7; ++r) a[7 * j + r] = tc::pack_h2(e0[r], e1[r]);
-        }
-        a_put<64, N0>(A, row, 0, a);
+        for (int j = 0; j < PA; ++j) encode_pair<NP>(scs, v, j, nk, c, a + 7 * j);
+        a_put<64, C1>(A, row, 0, a);
       } else {
-        constexpr int C1 = 7 * PA + FA / 2;           // first column of this thread's run
         constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
         constexpr int N1 = tc_k0p(NK) / 2 - C1;
+        static_assert(NE + NF + 1 <= N1, "the bias column is in thread 1's run");
         uint32_t a[N1];
 #pragma unroll
         for (int gq = 0; gq < (64 - FA) / 4; ++gq) {
@@ -339,17 +372,10 @@ geo_front_kernel(const DevScene* __restrict__ scp, const uint8_t* __restrict__ w
           a[NE + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
         }
 #pragma unroll
-        for (int j = PA; j < NP; ++j) {
-          float e0[7], e1[7];
-          encode_fast(scs, v, 2 * j, c, e0);
-          encode_fast(scs, v, 2 * j + 1, c, e1);
-#pragma unroll
-          for (int r = 0; r < 7; ++r) a[7 * (j - PA) + r] = tc::pack_h2(e0[r], e1[r]);
-        }
+        for (int j = PA; j < NP; ++j) encode_pair<NP>(scs, v, j, nk, c, a + 7 * (j - PA));
         a[NE + NF] = H2_ONE;
 #pragma unroll
         for (int i = NE + NF + 1; i < N1; ++i) a[i] = 0u;
-        static_assert(C1 % 4 == 0, "run starts on a 16-byte chunk");
         a_put<64, N1>(A, row, C1, a);
       }
     }
@@ -430,15 +456,15 @@ __device__ __forceinline__ void tail_mma(float* d, const uint8_t* ahi, const uin
   tc::named_sync(bar_id, 128);
 }
 
-template <int NK>
+// whi: the blob's W_hi tile of stage 4 (stage 5's follows it)
 __global__ void __launch_bounds__(GWG * 128, 1)
-geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wblob, const uint8_t* __restrict__ wlo, int lo_mask,
+geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ whi, const uint8_t* __restrict__ wlo, int lo_mask,
                 const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
                 const float* __restrict__ pool, int query_mode, ShadeOut so, uint4* __restrict__ lat_out) {
   extern __shared__ __align__(1024) uint8_t wsm[];
   __shared__ uint64_t wbar;
   __shared__ __align__(16) float wp2[132];                 // density head: w[0][64] | w[1][64] | b[2]
-  constexpr TcPlan plan = make_tc_plan(NK);
+  constexpr TcPlan plan = REL_PLAN;
   constexpr uint32_t HOFF = plan.st[4].off, WH = plan.st[GEO_NSTAGE].off - plan.st[4].off;   // W_hi of stages 4, 5
   const long long end = min((long long)*count_ptr, base + len);
   if (end <= base) return;
@@ -449,7 +475,7 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
   __syncthreads();
   if (t == 0) {   // [W_hi 4 | W_hi 5 | W_lo 4 | W_lo 5]
     tc::mbar_expect_tx(&wbar, 2 * WH);
-    tc::bulk_g2s(wsm, wblob + HOFF, WH, &wbar);
+    tc::bulk_g2s(wsm, whi, WH, &wbar);
     tc::bulk_g2s(wsm + WH, wlo, WH, &wbar);
     tc::mbar_wait(&wbar, 0, 0x31u);
   }
@@ -564,9 +590,9 @@ struct ColCtx {
   Group grp;
 };
 
-template <int NK, int STAGE>
+template <int STAGE>
 __device__ __forceinline__ void col_mma(const ColCtx& c) {
-  constexpr TcPlan plan = make_tc_plan(NK);
+  constexpr TcPlan plan = REL_PLAN;
   constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
   const uint32_t b = c.wbase + (plan.st[STAGE].off - plan.st[GEO_NSTAGE].off);
   wg_publish(c.bar_id);
@@ -613,7 +639,6 @@ __device__ __forceinline__ void col_epi(const ColCtx& c, const float* __restrict
 }
 
 // Colour pass for one tile of the second work list (entries: x = slot of the latent in the scratch buffer, y = sample id).
-template <int NK>
 __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, const SampleSrc& src,
                                            const int2* __restrict__ list2, const int* __restrict__ list1, int count, int tile,
                                            const ColCtx& cx, const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
@@ -677,7 +702,7 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
 #pragma unroll
     for (int i = 9; i < 16; ++i) a[i] = 0u;
     a_put<128, 16>(cx.A, cx.row, 0, a);
-    col_mma<NK, 12>(cx);
+    col_mma<12>(cx);
     float r[36];
     d_get<36>(cx, 0, r);
 #pragma unroll
@@ -709,10 +734,10 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     }
     a_put<128, 56>(cx.A, cx.row, 0, a);
   }
-  col_mma<NK, 6>(cx);
+  col_mma<6>(cx);
   // ---- BASE0 -> BASE1
   col_epi<2, 2>(cx, C.b_base0);
-  col_mma<NK, 7>(cx);
+  col_mma<7>(cx);
   float x[32];
   {
     float r[32];
@@ -724,10 +749,10 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * om, x[2 * i + 1] * om);  // vis_layer1(x * weight)
     a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  col_mma<NK, 8>(cx);
+  col_mma<8>(cx);
   // ---- VIS1A -> VIS1B (src/model.py:1294-1296)
   col_epi<1, 2>(cx, C.b_vis1a);
-  col_mma<NK, 9>(cx);
+  col_mma<9>(cx);
   {
     float r[36];
     d_get<36>(cx, 0, r);
@@ -739,7 +764,7 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * sg, x[2 * i + 1] * sg);  // x * sigmoid(vis) * mask
     a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  col_mma<NK, 10>(cx);
+  col_mma<10>(cx);
   // ---- VIS2A (+ 32->1 sigmoid on CUDA cores) -> OUT0 input [x32 | vis | ray_diff4 | 0-pad] (src/model.py:1297-1300)
   {
     float r[32];
@@ -758,7 +783,7 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
     for (int i = 19; i < 24; ++i) o[i] = 0u;
     a_put<128, 24>(cx.A, cx.row, 0, o);
   }
-  col_mma<NK, 11>(cx);
+  col_mma<11>(cx);
   // ---- OUT0 -> 16->8->1 on CUDA cores -> softmax over the views -> blended colour (src/model.py:1300-1301)
   float logit;
   {
@@ -787,32 +812,32 @@ __device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, 
   }
 }
 
-template <int NK>
+// wcol: the blob's tile of stage 6 (the colour stages' tiles follow it)
 __global__ void __launch_bounds__(CWG * 128, 1)
-shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wblob,
+shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wcol,
                    SampleSrc src, const int2* __restrict__ list2, const int* __restrict__ list1,
                    const int* __restrict__ count_ptr, const uint4* __restrict__ lat_in, int query_mode, ShadeOut so) {
   extern __shared__ __align__(1024) uint8_t wsm[];
   __shared__ uint64_t wbar;
   __shared__ SceneS scs;
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr uint32_t OFF0 = plan.st[GEO_NSTAGE].off, WBYTES = plan.total_bytes - plan.st[GEO_NSTAGE].off;
+  constexpr TcPlan plan = REL_PLAN;
+  constexpr uint32_t WBYTES = plan.total_bytes - plan.st[GEO_NSTAGE].off;
   constexpr uint32_t WPAD = (WBYTES + 1023u) / 1024u * 1024u;
   const int t = threadIdx.x, wg = t >> 7;
   const int count = *count_ptr;
   const int ntiles = (count + SPT - 1) / SPT;
   if (blockIdx.x * CWG >= ntiles) return;
-  stage_scene(scs, *scp, NK, t, CWG * 128);
+  stage_scene(scs, *scp, 0, t, CWG * 128);   // the colour head reads no keypoints
   if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
   __syncthreads();
-  if (t == 0) load_weights(wsm, wblob + OFF0, WBYTES, &wbar);   // the colour stages' weight tiles, once per CTA
+  if (t == 0) load_weights(wsm, wcol, WBYTES, &wbar);   // the colour stages' weight tiles, once per CTA
   __syncthreads();
   const int lane = t & 31;
   ColCtx cx{wsm + WPAD + (size_t)wg * (CA_BYTES + CD_BYTES), nullptr, tc::smem_u32(wsm), 1 + wg, t & 127, (t >> 5) & 3, lane,
             Group(lane)};
   cx.D = reinterpret_cast<float*>(cx.A + CA_BYTES);
   for (int tile = blockIdx.x * CWG + wg; tile < ntiles; tile += gridDim.x * CWG)
-    color_tile<NK>(scs, C, src, list2, list1, count, tile, cx, lat_in, query_mode, so);
+    color_tile(scs, C, src, list2, list1, count, tile, cx, lat_in, query_mode, so);
 }
 
 }  // namespace
@@ -823,29 +848,36 @@ size_t tc_weight_lo_bytes(int n_kpt) {
   return p.st[GEO_NSTAGE].off - p.st[4].off;
 }
 size_t tc_pool_bytes(long long n_max) { return (size_t)(n_max < POOL_SLICE ? n_max : POOL_SLICE) * POOL_W * sizeof(float); }
-bool tc_supported(int n_views, int n_kpt, int sp_level) { return n_views == 3 && (n_kpt == 18 || n_kpt == 24) && sp_level == 3; }
+bool tc_supported(int n_views, int n_kpt, int sp_level) {
+  return n_views == 3 && n_kpt >= 1 && n_kpt <= KPN_MAX_KPT && sp_level == 3;
+}
 
-template <int NK>
-static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask,
-                                  const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                                  const ShadeOut& so, uint4* lat, float* pool, int2* list2, int* count2, int num_sms,
+template <int NP>
+static cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo,
+                                  int lo_mask, const SampleSrc& src, const int* list, const int* counter, long long n_max,
+                                  int query_mode, const ShadeOut& so, uint4* lat, float* pool, int2* list2, int* count2, int num_sms,
                                   cudaEvent_t after_geo, int* launches, cudaStream_t st) {
+  constexpr int NK = 2 * NP, FWG = front_wgs(NK);
   constexpr TcPlan plan = make_tc_plan(NK);
-  const size_t smem_front = plan.st[4].off + (size_t)GWG * front_tile_bytes(NK);
-  const size_t smem_tail = 2 * (size_t)(plan.st[GEO_NSTAGE].off - plan.st[4].off) + (size_t)GWG * TAIL_TILE_BYTES;
-  const size_t smem_col = (plan.total_bytes - plan.st[GEO_NSTAGE].off + 1023) / 1024 * 1024 + (size_t)CWG * (CA_BYTES + CD_BYTES);
+  const size_t smem_front = front_smem_bytes(NK, FWG);
+  constexpr TcPlan rel = REL_PLAN;
+  constexpr uint32_t smem_tail = 2 * (rel.st[GEO_NSTAGE].off - rel.st[4].off) + GWG * TAIL_TILE_BYTES;
+  constexpr uint32_t smem_col = (rel.total_bytes - rel.st[GEO_NSTAGE].off + 1023) / 1024 * 1024 + CWG * (CA_BYTES + CD_BYTES);
   static std::atomic<bool> attr[64];   // function attributes are per device (zero-initialised; setting them twice is harmless)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
+    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(geo_tail_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
+    // the tail and colour kernels serve every keypoint count
+    e = cudaFuncSetAttribute(geo_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(shade_color_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_col);
+    e = cudaFuncSetAttribute(shade_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_col);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
+  const uint8_t* wtail = wblob + plan.st[4].off;
+  const uint8_t* wcol = wblob + plan.st[GEO_NSTAGE].off;
   auto grid_for = [&](long long tiles, int per_cta) {
     const long long g = (tiles + per_cta - 1) / per_cta;
     return (int)(g < 1 ? 1 : (g > num_sms ? num_sms : g));
@@ -855,10 +887,10 @@ static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const u
   const long long nslices = n_max > POOL_SLICE ? (n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
   for (long long s = 0; s < nslices; ++s) {
     const long long base = s * POOL_SLICE, len = n_max - base < POOL_SLICE ? n_max - base : POOL_SLICE;
-    geo_front_kernel<NK><<<grid_for((len + FSPT - 1) / FSPT, GWG), GWG * 128, smem_front, st>>>(sc, wblob, src, list, counter, base,
-                                                                                                  len, pool);
-    geo_tail_kernel<NK><<<grid_for((len + 63) / 64, GWG), GWG * 128, smem_tail, st>>>(C, wblob, wlo, lo_mask, list, counter, base,
-                                                                                       len, pool, query_mode, so, lat);
+    geo_front_kernel<NP><<<grid_for((len + FSPT - 1) / FSPT, FWG), FWG * 128, smem_front, st>>>(sc, nk, wblob, src, list, counter,
+                                                                                                  base, len, pool);
+    geo_tail_kernel<<<grid_for((len + 63) / 64, GWG), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len,
+                                                                                   pool, query_mode, so, lat);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     *launches += 2;
@@ -866,7 +898,7 @@ static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const u
   if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
   const int grid = grid_for((n_max + SPT - 1) / SPT, CWG);
   if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
-    shade_color_kernel<NK><<<grid, CWG * 128, smem_col, st>>>(sc, C, wblob, src, nullptr, list, counter, lat, query_mode, so);
+    shade_color_kernel<<<grid, CWG * 128, smem_col, st>>>(sc, C, wcol, src, nullptr, list, counter, lat, query_mode, so);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     *launches += 1;
@@ -877,10 +909,18 @@ static cudaError_t launch_tc_impl(const DevScene* sc, const TcConsts& C, const u
                                                                                                  list2, count2);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  shade_color_kernel<NK><<<grid, CWG * 128, smem_col, st>>>(sc, C, wblob, src, list2, nullptr, count2, lat, query_mode, so);
+  shade_color_kernel<<<grid, CWG * 128, smem_col, st>>>(sc, C, wcol, src, list2, nullptr, count2, lat, query_mode, so);
   *launches += 2;
   return cudaGetLastError();
 }
+
+using LaunchTc = decltype(&launch_tc_impl<1>);
+template <int... I>
+static constexpr std::array<LaunchTc, sizeof...(I)> launch_table(std::integer_sequence<int, I...>) {
+  return {&launch_tc_impl<I + 1>...};
+}
+// launch_tc_impl<NP> for NP = 1 .. KPN_MAX_KPT / 2 keypoint pairs
+static constexpr std::array<LaunchTc, KPN_MAX_KPT / 2> LAUNCH_TC = launch_table(std::make_integer_sequence<int, KPN_MAX_KPT / 2>{});
 
 cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term, int n_kpt,
                             const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
@@ -888,11 +928,10 @@ cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t
                             cudaEvent_t after_geo, int* launches, cudaStream_t st) {
   // W_lo and A_lo passes of the density tail (stages 4, 5: bits 4, 5 and 6, 7); single-term weights keep the A_lo passes
   const int lo_mask = two_term ? 0xF0 : 0xC0;
-  if (n_kpt == 18)
-    return launch_tc_impl<18>(sc, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
-                              (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo, launches, st);
-  return launch_tc_impl<24>(sc, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so, (uint4*)lat_scratch,
-                            (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo, launches, st);
+  if (n_kpt < 1 || n_kpt > KPN_MAX_KPT) return cudaErrorInvalidValue;
+  return LAUNCH_TC[tc_npair(n_kpt) - 1](sc, n_kpt, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so,
+                                        (uint4*)lat_scratch, (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo,
+                                        launches, st);
 }
 
 // Watchdog state of this module's kernels: out[0] != 0 -> some barrier wait gave up at block out[1], thread out[2], tag out[3].

@@ -26,20 +26,41 @@ struct TcPlan {
   int K0P;  // padded input width of layer 0
 };
 
+// keypoint pairs of the layer-0 input: keypoints 2j and 2j+1 share the fp16 words of pair j; with an odd count the last
+// pair's second slot has no weights (the blob is zero there) and the kernel writes 0 into it
+__host__ __device__ constexpr int tc_npair(int n_kpt) { return (n_kpt + 1) / 2; }
 // layer-0 input width incl. the bias row, padded to a multiple of 16
-__host__ __device__ constexpr int tc_k0p(int n_kpt) { return ((7 * n_kpt + 64 + 1) + 15) / 16 * 16; }
-// split of the layer-0 input between the two threads of a row: thread 0 builds keypoint pairs [0, PA) and feature
-// channels [0, FA), thread 1 the remaining pairs, the remaining channels and the bias column
-// (18 keypoints: 4 | 5 pairs; 24: 4 | 8 pairs -- the second thread starts a tile earlier, its partner writes the tile's outputs;
-// the 40 | 24 channel split keeps one gather plan for both keypoint counts: 10 | 6 float4 groups of feat64)
-__host__ __device__ constexpr int tc_l0_pa(int n_kpt) { return 4 + 0 * n_kpt; }
-__host__ __device__ constexpr int tc_l0_fa(int n_kpt) { return 40 + 0 * n_kpt; }
+__host__ __device__ constexpr int tc_k0p(int n_kpt) { return ((14 * tc_npair(n_kpt) + 64 + 1) + 15) / 16 * 16; }
+
+// Split of the layer-0 input between the two threads of a row: thread 0 builds keypoint pairs [0, pa) and feature channels
+// [0, fa) as words [0, 7*pa + fa/2), thread 1 the remaining pairs, the remaining channels and the bias column from there on.
+// Both runs start on a 16-byte chunk: 7*pa + fa/2 = 0 (mod 4) with fa a multiple of 4 (float4 groups of feat64), so pa is
+// even.  The split depends on the pair count only (an odd count shares its even neighbour's kernel) and balances the two
+// runs' words; 17/18 and 23/24 keypoints keep the 4 | 40 split the engine has always used for 18 and 24 (another split
+// permutes the K order of layer 0, which changes the last bits of its sums).
+struct TcSplit { int pa, fa; };
+__host__ __device__ constexpr TcSplit tc_l0_split(int n_kpt) {
+  const int np = tc_npair(n_kpt);
+  if (np == 9 || np == 12) return TcSplit{4, 40};
+  const int half = tc_k0p(n_kpt) / 4;   // words per thread of an even split
+  TcSplit best{0, 0};
+  int best_d = 1 << 30;
+  for (int pa = 0; pa <= np; pa += 2)
+    for (int fa = 0; fa <= 64; fa += 4) {
+      const int c1 = 7 * pa + fa / 2;
+      const int d = c1 > half ? c1 - half : half - c1;
+      if (c1 % 4 == 0 && d < best_d) { best = TcSplit{pa, fa}; best_d = d; }
+    }
+  return best;
+}
+__host__ __device__ constexpr int tc_l0_pa(int n_kpt) { return tc_l0_split(n_kpt).pa; }
+__host__ __device__ constexpr int tc_l0_fa(int n_kpt) { return tc_l0_split(n_kpt).fa; }
 
 // K index (fp16 element of the activation row) that input `i` of geometry stage `stage` is multiplied with.
 // Stage 0 inputs: i < 7*n_kpt is encoding element r*n_kpt + k (reference src/spatial.py layout), else feat64 channel.
 __host__ __device__ constexpr int tc_kmap(int stage, int n_kpt, int i) {
   if (stage != 0) return i;
-  const int NP = n_kpt / 2, PA = tc_l0_pa(n_kpt), FA = tc_l0_fa(n_kpt);
+  const int NP = tc_npair(n_kpt), PA = tc_l0_pa(n_kpt), FA = tc_l0_fa(n_kpt);
   if (i < 7 * n_kpt) {
     const int r = i / n_kpt, k = i % n_kpt, j = k / 2;
     const int col = j < PA ? 7 * j + r : 7 * PA + FA / 2 + 7 * (j - PA) + r;
@@ -51,7 +72,7 @@ __host__ __device__ constexpr int tc_kmap(int stage, int n_kpt, int i) {
 // K index of the bias row of a geometry stage (or of stage 12)
 __host__ __device__ constexpr int tc_kbias(int stage, int n_kpt) {
   switch (stage) {
-    case 0: return 2 * (7 * (n_kpt / 2) + 32);
+    case 0: return 2 * (7 * tc_npair(n_kpt) + 32);
     case 1: return 128;
     case 2: return 136;
     case 3: return 120;
