@@ -74,7 +74,7 @@ typedef struct {
 /* Source-side inputs of KeypointNeRF.query (reference src/model.py:690-782): cam dict,
  * sp_data, cached feature maps, source images and foreground masks. */
 typedef struct {
-  int n_views, n_kpt;
+  int n_views, n_kpt;            /* 1 <= n_views <= KPN_MAX_VIEWS (engine 0 / 2-4: 3 or 4 views; engine 1: any) */
   float src_width, src_height;   /* cam["width"], cam["height"] */
   float znear, zfar;             /* cam["znear"], cam["zfar"] */
   float nml_scale;               /* cam["nml_scale"] */
@@ -121,7 +121,7 @@ typedef struct {
   int engine;             /* 0 = default: tensor cores (wgmma), fp16 operands, fp32 accumulate; the density tail (stages P0|compress,
                                  P1) runs with two-term (hi+lo) weights and activations;
                              1 = fp32 CUDA-core engine (parity anchor, ~25x slower; the ONLY engine for shapes the tensor-core
-                                 engine does not cover: n_views != 3, sp_level != 3 -- such shapes fail with
+                                 engine does not cover: n_views 1 or 2, sp_level != 3 -- such shapes fail with
                                  KPN_ERR_UNSUPPORTED unless engine = 1 is requested explicitly).  Every engine takes any
                                  1 <= n_kpt <= KPN_MAX_KPT;
                              2 = as 0 with single-term fp16 weights in the density tail (more rounding error);

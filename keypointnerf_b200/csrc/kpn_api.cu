@@ -119,11 +119,12 @@ extern "C" int kpn_create(int device, kpn_ctx** out) {
   if (!ok) { kpn_destroy(c); return KPN_ERR_CUDA; }
   cudaMemset(c->d_counters, 0, sizeof(int) * MAX_CHUNKS);
   cudaMemset(c->d_counters2, 0, sizeof(int) * MAX_CHUNKS);
-  if (cudaHostAlloc(reinterpret_cast<void**>(&c->h_wd), 8 * sizeof(unsigned int), cudaHostAllocDefault) != cudaSuccess) {
+  const size_t wd_bytes = TC_WD_MODULES * TC_WD_WORDS * sizeof(unsigned int);
+  if (cudaHostAlloc(reinterpret_cast<void**>(&c->h_wd), wd_bytes, cudaHostAllocDefault) != cudaSuccess) {
     kpn_destroy(c);
     return KPN_ERR_CUDA;
   }
-  memset(c->h_wd, 0, 8 * sizeof(unsigned int));
+  memset(c->h_wd, 0, wd_bytes);
   *out = c;
   return KPN_OK;
 }
@@ -155,10 +156,14 @@ extern "C" const char* kpn_last_error(const kpn_ctx* c) { return c ? c->err.c_st
 // by looking at the last copy that has landed (wd_check): a raised flag is reported ONCE as KPN_ERR_CUDA and cleared on the
 // device (stream-ordered), which re-arms the engine for the calls that follow.
 static int wd_check(kpn_ctx* c, cudaStream_t st) {
-  volatile unsigned int* w = c->h_wd;
-  if (!w || w[0] == 0u) return KPN_OK;
+  volatile unsigned int* w = nullptr;   // the words of the first module whose flag is raised
+  for (int m = TC_WD_MODULES - 1; c->h_wd && m >= 0; --m) {
+    volatile unsigned int* wm = c->h_wd + TC_WD_WORDS * m;
+    if (wm[0] != 0u) w = wm;
+  }
+  if (!w) return KPN_OK;
   const unsigned int blk = w[1], thr = w[2], tag = w[3], par = w[4];
-  for (int i = 0; i < 8; ++i) c->h_wd[i] = 0u;
+  for (int i = 0; i < TC_WD_MODULES * TC_WD_WORDS; ++i) c->h_wd[i] = 0u;
   KPN_CUDA(c, tc_watchdog_clear_async(st));
   KPN_FAIL(c, KPN_ERR_CUDA, "device watchdog: a barrier wait of a tensor-core kernel gave up (block %u, thread %u, tag 0x%x, parity %u); "
            "the results of that call (and of tensor-core calls enqueued after it) are invalid; the flag has been cleared",
@@ -297,7 +302,8 @@ extern "C" int kpn_set_scene(kpn_ctx* c, const kpn_scene* s, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (!c->have_weights) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_weights must precede kpn_set_scene");
   { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  if (s->n_views < 1 || s->n_views > 3) KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "n_views=%d unsupported (1..3)", s->n_views);
+  if (s->n_views < 1 || s->n_views > KPN_MAX_VIEWS)
+    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "n_views=%d unsupported (1..%d)", s->n_views, KPN_MAX_VIEWS);
   if (s->n_kpt != c->n_kpt) KPN_FAIL(c, KPN_ERR_ARG, "scene n_kpt=%d != weights n_kpt=%d", s->n_kpt, c->n_kpt);
   if (!s->KRT || !s->extrin || !s->kpt3d || !s->bounds || !s->feat64 || !s->feat8 || !s->feat_tex || !s->img)
     KPN_FAIL(c, KPN_ERR_ARG, "null scene pointer");
@@ -381,7 +387,7 @@ static int shade_batch(kpn_ctx* c, const SampleSrc& src, const int* list, const 
   const bool use_tc = engine != 1;
   if (engine < 0 || engine > 4) KPN_FAIL(c, KPN_ERR_ARG, "kpn_opts.engine = %d (0 .. 4)", engine);
   if (use_tc && !(c->tc_weights && tc_supported(c->scene_views, c->n_kpt, c->sp_level)))
-    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "the tensor-core engine covers n_views == 3, 1 <= n_kpt <= %d, sp_level == 3; this scene has "
+    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "the tensor-core engine covers n_views 3 or 4, 1 <= n_kpt <= %d, sp_level == 3; this scene has "
              "n_views=%d n_kpt=%d sp_level=%d: request engine = 1 (fp32 CUDA-core engine, ~25x slower) explicitly",
              KPN_MAX_KPT, c->scene_views, c->n_kpt, c->sp_level);
   cudaEvent_t e0 = nullptr, em = nullptr, e1 = nullptr;   // start | after the geometry kernel | stop
@@ -400,13 +406,13 @@ static int shade_batch(kpn_ctx* c, const SampleSrc& src, const int* list, const 
     KPN_CUDA(c, c->ws_list2.reserve((size_t)n * 8));
     KPN_CUDA(c, c->ws_pool.reserve(tc_pool_bytes(n)));
     int launches = 0;
-    KPN_CUDA(c, launch_shade_tc(c->d_scene, c->tcc, c->wblob.as<uint8_t>(), c->wlo.as<uint8_t>(), engine == 2 ? 0 : 1, c->n_kpt, src,
+    KPN_CUDA(c, launch_shade_tc(c->d_scene, c->scene_views, c->tcc, c->wblob.as<uint8_t>(), c->wlo.as<uint8_t>(), engine == 2 ? 0 : 1, c->n_kpt, src,
                                 list, counter, n, query_mode, so, c->ws_lat.p, c->ws_pool.p, c->ws_list2.p, counter2, c->num_sms, em,
                                 &launches, st));
     c->launches += launches;
   }
   else {
-    KPN_CUDA(c, launch_shade_simt(c->d_scene, c->d_wf32, src, list, counter, n, query_mode, so, c->num_sms, st));
+    KPN_CUDA(c, launch_shade_simt(c->d_scene, c->scene_views, c->d_wf32, src, list, counter, n, query_mode, so, c->num_sms, st));
     if (c->profiling) KPN_CUDA(c, cudaEventRecord(em, st));
     c->launches++;
   }

@@ -404,10 +404,10 @@ __global__ void compact_kernel(const DevScene* __restrict__ sc, SampleSrc src, l
 }
 
 // ------------------------------------------------------------------------------------------------
-// shade (fp32 SIMT): tiles of 64 valid samples, 256 threads
+// shade (fp32 SIMT): tiles of TS valid samples, 4 TS threads.  The view-indexed shared arrays hold NV views: up to 3 views in
+// tiles of 64 samples, 4 views in tiles of 56 (64 samples x 4 views would need 253 952 B of shared memory).  A sample's
+// arithmetic does not depend on the tile it sits in.
 // ------------------------------------------------------------------------------------------------
-constexpr int TS = 64;
-constexpr int NT = 256;
 constexpr int LDA = 7 * MAXK + 64;  // widest geometry input (7*KPN_MAX_KPT encodings + feat64) = 288 floats, multiple of 4
 static_assert(LDA % 4 == 0, "rows are read as float4");
 constexpr int LDB = 128;
@@ -421,7 +421,7 @@ __device__ __forceinline__ float apply_act(float x) {
   return x;
 }
 
-// out[r][n] = act(bias[n] + sum_k in[r][k] * Wt[k][n]) for the 64 rows of the tile.
+// out[r][n] = act(bias[n] + sum_k in[r][k] * Wt[k][n]) for the rows of the tile (8 per warp).
 // Warp w owns rows 8w..8w+7 (A operand is a warp-wide broadcast), lane owns columns lane+32j.
 template <int ACT, int NJ>
 __device__ __forceinline__ void dense_tile(const DevWeightsF32& W, int L, const float* sIn, int ldi, float* sOut, int ldo) {
@@ -479,49 +479,56 @@ __device__ __forceinline__ void dense_tile(const DevWeightsF32& W, int L, const 
 struct ShadeSmem {
   float* A;     // [TS][LDA]
   float* B;     // [TS][LDB]
-  float* XV;    // [3][TS][64]   (later scratch S1,S2,S3)
-  float* F;     // [3][TS][36]
+  float* XV;    // [NV][TS][64]   (later scratch S1,S2,S3)
+  float* F;     // [NV][TS][36]
   float* MV;    // [TS][72]
   float* Lat;   // [TS][24]
-  float* RD;    // [3][TS][4]
-  float* RGB;   // [3][TS][4]
-  float* UV;    // [3][TS][4]  u, v, zn, boundary weight
-  float* PW;    // [3][TS]
-  float* Om;    // [3][TS]
+  float* RD;    // [NV][TS][4]
+  float* RGB;   // [NV][TS][4]
+  float* UV;    // [NV][TS][4]  u, v, zn, boundary weight
+  float* PW;    // [NV][TS]
+  float* Om;    // [NV][TS]
   float* P;     // [TS][8]  p xyz, d xyz
   float* F8;    // [TS][8]
   float* Geo;   // [TS][2]
   float* Vis;   // [TS]
-  float* Logit; // [3][TS]
+  float* Logit; // [NV][TS]
   int* Id;      // [TS]
 };
 
-constexpr int SHADE_SMEM_FLOATS = TS * LDA + TS * LDB + 3 * TS * 64 + 3 * TS * 36 + TS * 72 + TS * 24 + 3 * TS * 4 * 3 +
-                                  3 * TS * 2 + TS * 8 * 2 + TS * 2 + TS + 3 * TS + TS;
-constexpr size_t SHADE_SMEM_BYTES = SHADE_SMEM_FLOATS * sizeof(float);
+__host__ __device__ constexpr int shade_smem_floats(int NV, int TS) {
+  return TS * LDA + TS * LDB + NV * TS * 64 + NV * TS * 36 + TS * 72 + TS * 24 + NV * TS * 4 * 3 + NV * TS * 2 + TS * 8 * 2 +
+         TS * 2 + TS + NV * TS + TS;
+}
+template <int NV, int TS>
+constexpr size_t SHADE_SMEM_BYTES = shade_smem_floats(NV, TS) * sizeof(float);
+static_assert(SHADE_SMEM_BYTES<3, 64> <= 227u * 1024u && SHADE_SMEM_BYTES<4, 56> <= 227u * 1024u, "fp32 engine tiles");
+static_assert(MAXV == 4, "the fp32 engine's tiles cover up to 4 views");
 
-__global__ void __launch_bounds__(NT, 1)
+template <int NV, int TS>
+__global__ void __launch_bounds__(4 * TS, 1)
 shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restrict__ Wp, SampleSrc src,
                   const int* __restrict__ list, const int* __restrict__ count_ptr, int query_mode, ShadeOut so) {
+  constexpr int NT = 4 * TS;
   extern __shared__ float4 smem4[];
   float* sm = reinterpret_cast<float*>(smem4);
   ShadeSmem s;
   s.A = sm; sm += TS * LDA;
   s.B = sm; sm += TS * LDB;
-  s.XV = sm; sm += 3 * TS * 64;
-  s.F = sm; sm += 3 * TS * 36;
+  s.XV = sm; sm += NV * TS * 64;
+  s.F = sm; sm += NV * TS * 36;
   s.MV = sm; sm += TS * 72;
   s.Lat = sm; sm += TS * 24;
-  s.RD = sm; sm += 3 * TS * 4;
-  s.RGB = sm; sm += 3 * TS * 4;
-  s.UV = sm; sm += 3 * TS * 4;
-  s.PW = sm; sm += 3 * TS;
-  s.Om = sm; sm += 3 * TS;
+  s.RD = sm; sm += NV * TS * 4;
+  s.RGB = sm; sm += NV * TS * 4;
+  s.UV = sm; sm += NV * TS * 4;
+  s.PW = sm; sm += NV * TS;
+  s.Om = sm; sm += NV * TS;
   s.P = sm; sm += TS * 8;
   s.F8 = sm; sm += TS * 8;
   s.Geo = sm; sm += TS * 2;
   s.Vis = sm; sm += TS;
-  s.Logit = sm; sm += 3 * TS;
+  s.Logit = sm; sm += NV * TS;
   s.Id = reinterpret_cast<int*>(sm);
   float* S1 = s.XV;
   float* S2 = s.XV + TS * 64;
@@ -960,20 +967,29 @@ cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n
   compact_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(sc, src, n, list, counter, out5, valid_out);
   return cudaGetLastError();
 }
-cudaError_t launch_shade_simt(const DevScene* sc, const DevWeightsF32* W, const SampleSrc& src, const int* list,
-                              const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
-                              cudaStream_t st) {
+template <int NV, int TS>
+static cudaError_t launch_shade_simt_tile(const DevScene* sc, const DevWeightsF32* W, const SampleSrc& src, const int* list,
+                                          const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
+                                          cudaStream_t st) {
+  constexpr size_t smem = SHADE_SMEM_BYTES<NV, TS>;
   static std::atomic<bool> attr_set[64];   // function attributes are per device (setting them twice is harmless)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(shade_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SHADE_SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(shade_simt_kernel<NV, TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
   int grid = grid_for(n_max, TS, num_sms);
-  shade_simt_kernel<<<grid, NT, SHADE_SMEM_BYTES, st>>>(sc, W, src, list, counter, query_mode, so);
+  shade_simt_kernel<NV, TS><<<grid, 4 * TS, smem, st>>>(sc, W, src, list, counter, query_mode, so);
   return cudaGetLastError();
+}
+cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,
+                              const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
+                              cudaStream_t st) {
+  if (n_views < 1 || n_views > MAXV) return cudaErrorInvalidValue;
+  return n_views <= 3 ? launch_shade_simt_tile<3, 64>(sc, W, src, list, counter, n_max, query_mode, so, num_sms, st)
+                      : launch_shade_simt_tile<4, 56>(sc, W, src, list, counter, n_max, query_mode, so, num_sms, st);
 }
 cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb, const int* start0, const int* cnt0,
                              const int* start1, const int* cnt1, const float* zbuf, const float* ray_nf, int r0, int nr, int S,

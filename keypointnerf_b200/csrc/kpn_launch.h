@@ -14,7 +14,7 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr
                          cudaStream_t st);
 cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out5,
                            uint8_t* valid_out, cudaStream_t st);
-cudaError_t launch_shade_simt(const DevScene* sc, const DevWeightsF32* W, const SampleSrc& src, const int* list,
+cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,
                               const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
                               cudaStream_t st);
 cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb, const int* start0, const int* cnt0,
@@ -24,17 +24,27 @@ cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb
 cudaError_t launch_resample(const int* list, const float* cw, const int* start0, const int* cnt0, const int* start1, const int* cnt1,
                             const float* ray_nf, int nr, int Sc, int Sf, float* zout, float* contrib_out, cudaStream_t st);
 // Tensor-core engine: geometry front (L0-L3 + pooling) and density tail kernels, then the colour kernel on the samples with
-// density > 0.  wblob: full fp16 W_hi tiles of every stage; wlo: W_lo tiles of stages 4, 5 (tc_weight_lo_bytes);
-// lat_scratch: n_max x 48 bytes, pool_scratch: tc_pool_bytes(n_max), list2: n_max x int2, count2: device int (zeroed by the
-// caller).  *launches is incremented by the number of kernels enqueued.
-cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term, int n_kpt,
-                            const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
+// density > 0.  n_views: 3 or 4 (the scene's view count, tc_supported); wblob: full fp16 W_hi tiles of every stage; wlo: W_lo
+// tiles of stages 4, 5 (tc_weight_lo_bytes); lat_scratch: n_max x 48 bytes, pool_scratch: tc_pool_bytes(n_max), list2:
+// n_max x int2, count2: device int (zeroed by the caller).  *launches is incremented by the number of kernels enqueued.
+cudaError_t launch_shade_tc(const DevScene* sc, int n_views, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term,
+                            int n_kpt, const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
                             const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
                             cudaEvent_t after_geo, int* launches, cudaStream_t st);
+// the 4-view instantiation (kpn_shade_tc_v4.cu); lo_mask as launch_shade_tc derives it from two_term
+cudaError_t launch_shade_tc_v4(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask, int n_kpt,
+                               const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
+                               const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
+                               cudaEvent_t after_geo, int* launches, cudaStream_t st);
 size_t tc_pool_bytes(long long n_max);
-cudaError_t tc_watchdog_read(unsigned int out[8], bool reset);
-cudaError_t tc_watchdog_read_async(unsigned int* pinned_out8, cudaStream_t st);   // stream-ordered copy into pinned host memory
+// Device watchdog words of the tensor-core kernels: TC_WD_WORDS per module, one module per view-count translation unit.
+constexpr int TC_WD_WORDS = 8;
+constexpr int TC_WD_MODULES = 2;
+cudaError_t tc_watchdog_read(unsigned int out[8], bool reset);   // the first module whose flag is raised (else the first module)
+// stream-ordered copy of every module's words into pinned host memory (TC_WD_MODULES x TC_WD_WORDS)
+cudaError_t tc_watchdog_read_async(unsigned int* pinned_out, cudaStream_t st);
 cudaError_t tc_watchdog_clear_async(cudaStream_t st);
+cudaError_t tc_watchdog_addr_v4(void** p);   // device address of the 4-view module's words
 cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles);   // not supported: cudaErrorNotSupported
 size_t tc_weight_blob_bytes(int n_kpt);
 size_t tc_weight_lo_bytes(int n_kpt);

@@ -1,164 +1,10 @@
-// Ray-march shading, engine 0: Hopper tensor-core MLPs (wgmma, fp16 operands in shared memory, fp32 accumulators in
-// registers, weights resident in shared memory through one bulk-TMA load per CTA).
-//
-// Three persistent kernels per batch of valid samples:
-//   geo_front_kernel  : gather + keypoint encoding + geometry MLP (L0-L3) + view pooling.  A row is one (sample, source view)
-//                       pair; the 3 views of a sample sit in 3 adjacent lanes (10 samples per warp), so the pooling (reference
-//                       src/utils.py:722-748) is a 3-lane shuffle.  Writes the pooled [mean | var] (fp32) of every sample to a
-//                       scratch buffer.
-//   geo_tail_kernel   : density tail per sample (P0|compress, P1 with two-term fp16 weights W_hi + W_lo and two-term
-//                       activations, 64->2 head in fp32).  Writes alpha/sdf and, where a colour is needed, the 24-wide
-//                       compressed latent (fp16).  The tail is a kernel of its own because the geometry stages' W_hi tiles and
-//                       the tail's W_hi + W_lo tiles do not fit in one SM's 227 KB of shared memory together with the tiles.
-//   shade_color_kernel: IBR colour head (RE1, BASE0, BASE1, VIS1A, VIS1B, VIS2A, OUT0 on tensor cores; first ray-encoder layer,
-//                       32->1, 16->8->1 in fp32 on CUDA cores) for the samples with density > 0 (colour_list_kernel's list).
-// Common structure: a warpgroup (4 warps) owns a tile of rows.  Row threads build a layer input as packed fp16 pairs in an
-// activation tile in shared memory (tc::a_word_off layout), the warpgroup multiplies it with the resident weights
-// (wgmma.mma_async, M = 64 per instruction), and the epilogue either runs on the accumulator fragments directly (elementwise
-// activations, written straight into the next layer's activation tile) or stores them to shared memory for the row threads
-// (cross-view reductions).  Biases ride in the MMAs as one extra K row multiplied by a constant 1 in the activation tile.
-// Stage table:
-//   geo    0 L0 190->128 | 1 L1 128->128 | 2 L2 136->120 | 3 L3 120->64 | 4 P0|CMP 128->64|24 | 5 P1 64->64
-//   colour 12 RE1 16->35 | 6 BASE0 105->64 | 7 BASE1 64->32 | 8 VIS1A 32->32 | 9 VIS1B 32->33 | 10 VIS2A 32->32 | 11 OUT0 37->16
-#include <array>
-#include <atomic>
-#include <cstdlib>
-#include <type_traits>
-#include <utility>
-#include "kpn_device.cuh"
-#include "kpn_launch.h"
-#include "kpn_tc.cuh"
-#include "kpn_tc_types.cuh"
+// Tensor-core engine (kpn_shade_tc.cuh): the 3-view instantiations of the view-dependent kernels, the kernels every view count
+// shares (density tail, colour work list) and the host entry points.  The 4-view kernels are in kpn_shade_tc_v4.cu, a translation
+// unit of their own so that the two sets of 16 front-kernel variants compile in parallel.
+#include "kpn_shade_tc.cuh"
 
 namespace kpn {
 namespace {
-
-constexpr int ROW_WARPS = 4;                              // warps of a warpgroup
-constexpr int GEO_NSTAGE = 6;                             // colour stages start at plan.st[6]
-constexpr int SPW = 10;                                   // samples per warp (3 views each)
-constexpr int SPT = SPW * ROW_WARPS;                      // samples per colour tile (128 rows)
-constexpr float LOG2E = 1.4426950408889634f;
-constexpr unsigned FULL = 0xffffffffu;
-
-__device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float lg2f(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float rcpf(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-
-// Softplus(beta=100): max(x,0) + log1p(exp(-100|x|))/100  (reference src/utils.py:523-524; beyond the
-// reference's threshold the correction term is < 2e-11).
-__device__ __forceinline__ float sp_fast(float x) {
-  float e = ex2f(-100.0f * LOG2E * fabsf(x));
-  return fmaf(0.0069314718056f, lg2f(1.0f + e), fmaxf(x, 0.0f));
-}
-__device__ __forceinline__ float elu_fast(float x) { return x > 0.0f ? x : ex2f(x * LOG2E) - 1.0f; }
-__device__ __forceinline__ float sig_fast(float x) { return rcpf(1.0f + ex2f(-x * LOG2E)); }
-__device__ __forceinline__ float u2f(uint32_t u) { return __uint_as_float(u); }
-
-// two-term fp16 split of a pair of activations: hi = fp16(x), lo = fp16(x - hi)
-__device__ __forceinline__ void split_h2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  __half2 h = __floats2half2_rn(a, b);
-  float2 f = __half22float2(h);
-  __half2 l = __floats2half2_rn(a - f.x, b - f.y);
-  hi = *reinterpret_cast<uint32_t*>(&h);
-  lo = *reinterpret_cast<uint32_t*>(&l);
-}
-
-// Scene constants the row threads need, staged once per CTA in shared memory (the per-view index differs per lane).
-struct SceneS {
-  float P[3][12];   // KRT rows
-  float E[3][12];   // extrinsic rows
-  float C[3][4];    // source camera centres
-  float4 kc[3][KPN_MAX_KPT];   // keypoints in camera space
-  float wm1, hm1, znear, inv_zrange, sp_scale, inv2sig2, inv_wm1, inv_hm1;
-  MapDesc f64, f8, ftex, img;
-};
-
-__device__ __forceinline__ Proj project_s(const SceneS& S, int v, const float p[3]) {
-  const float* P = S.P[v];
-  float hx = P[0] * p[0] + P[1] * p[1] + P[2] * p[2] + P[3];
-  float hy = P[4] * p[0] + P[5] * p[1] + P[6] * p[2] + P[7];
-  float hz = P[8] * p[0] + P[9] * p[1] + P[10] * p[2] + P[11];
-  Proj r;
-  r.u = 2.0f * ((hx / hz) / S.wm1) - 1.0f;
-  r.v = 2.0f * ((hy / hz) / S.hm1) - 1.0f;
-  r.zn = 2.0f * (hz - S.znear) * S.inv_zrange - 1.0f;
-  return r;
-}
-__device__ __forceinline__ float boundary_weight_fast(const Proj& q) {
-  float c[3] = {q.u, q.v, q.zn};
-  float w = 1.0f;
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    float x = 0.5f * c[i] + 0.5f;
-    float db = fminf(x, 1.0f - x);
-    w *= sig_fast(fmaf(50.0f, db, -5.0f));   // sigmoid(5*(db/0.1 - 1)), reference src/model.py:755
-  }
-  return w;
-}
-
-// Keypoint encoding of one keypoint with sp_level == 3: sin/cos(pi*2^l*dz) from one sincos + double angles.
-__device__ __forceinline__ void encode_fast(const SceneS& S, int v, int k, const float c[3], float e[7]) {
-  const float4 kc = S.kc[v][k];
-  float dx = c[0] - kc.x, dy = c[1] - kc.y, dzc = c[2] - kc.z;
-  float dz = S.sp_scale * dzc;
-  float w = __expf(-(dx * dx + dy * dy + dzc * dzc) * S.inv2sig2);
-  // sin/cos(pi * dz) have period 2 in dz: reduce to [-1, 1] first, so that the fast intrinsic stays accurate for any scale of the
-  // scene (sp_args.sigma = 150 / millimetre scenes make |dz| large; with metres and sigma = 0.1 the reduction is the identity)
-  const float dr = fmaf(-2.0f, rintf(0.5f * dz), dz);
-  float s, co;
-  __sincosf(dr * 3.14159265358979f, &s, &co);
-  float s2 = 2.0f * s * co, c2 = 1.0f - 2.0f * s * s;
-  float s4 = 2.0f * s2 * c2, c4 = 1.0f - 2.0f * s2 * s2;
-  e[0] = dz * w; e[1] = s * w; e[2] = co * w; e[3] = s2 * w; e[4] = c2 * w; e[5] = s4 * w; e[6] = c4 * w;
-}
-
-constexpr uint32_t H2_ONE = 0x00003C00u;   // fp16 pair (1.0, 0.0): the activation column that multiplies the bias row
-
-// softplus(beta=100) of two accumulators -> packed fp16 pair, on packed halves and WITHOUT the special-function unit: x is
-// rounded to fp16 first (the result is an fp16 activation anyway), y = max(x,0) + c(|x|) with the correction
-// c(t) = log1p(exp(-100 t))/100 ~ q^3 (a0 + a1 q + a2 q^2), q = sat(1 - t/0.08)  (minimax fit, fp16 coefficients): 8 instructions
-// per pair (F2FP, HFMA2.SAT, 2 HMUL2, 3 HFMA2, HMNMX2).  Against the exact softplus over every fp16 input the error is
-// <= 2.8e-5 (rms 9e-6; rounding the exact result to fp16 alone: 1.9e-5 / 2.5e-6), and the rendered RGB error is unchanged
-// (tools/err_budget.py: 7.6e-4 vs 7.7e-4 max on the bench-scene tile).  The previous form took one MUFU.EX2 per ELEMENT; at 4
-// lanes/clk/quarter the three 128-wide epilogues of a tile kept the XU pipe busy for 1.5k cycles per warp and throttled MIO.
-__device__ __forceinline__ uint32_t sp_pair(uint32_t a0, uint32_t a1) {
-  const __half2 xh = __floats2half2_rn(u2f(a0), u2f(a1));
-  const uint32_t k_it = 0xca40ca40u;   // -12.5 = -1 / 0.08
-  const uint32_t k_one = 0x3c003c00u;
-  const uint32_t a2 = 0x24c724c7u, a1c = 0xa459a459u, a0c = 0x1d631d63u;   // 0.018666, -0.016988, 0.00526 (fp16)
-  const uint32_t xa = *reinterpret_cast<const uint32_t*>(&xh) & 0x7fff7fffu;   // |x| (folds into the HFMA2 as an operand modifier)
-  uint32_t q;
-  asm("fma.rn.sat.f16x2 %0, %1, %2, %3;" : "=r"(q) : "r"(xa), "r"(k_it), "r"(k_one));
-  const __half2 qh = *reinterpret_cast<const __half2*>(&q);
-  const __half2 q2 = __hmul2(qh, qh);
-  const __half2 q3 = __hmul2(q2, qh);
-  __half2 p = __hfma2(*reinterpret_cast<const __half2*>(&a2), qh, *reinterpret_cast<const __half2*>(&a1c));
-  p = __hfma2(p, qh, *reinterpret_cast<const __half2*>(&a0c));
-  const uint32_t zero = 0u;
-  const __half2 y = __hfma2(p, q3, __hmax2(xh, *reinterpret_cast<const __half2*>(&zero)));
-  return *reinterpret_cast<const uint32_t*>(&y);
-}
-
-__device__ __forceinline__ void stage_scene(SceneS& scs, const DevScene& g, int NK, int t, int nthreads) {
-  for (int i = t; i < 3 * 12; i += nthreads) { scs.P[i / 12][i % 12] = g.P[i / 12][i % 12]; scs.E[i / 12][i % 12] = g.E[i / 12][i % 12]; }
-  for (int i = t; i < 3 * 3; i += nthreads) scs.C[i / 3][i % 3] = g.C[i / 3][i % 3];
-  for (int i = t; i < 3 * NK; i += nthreads)
-    scs.kc[i / NK][i % NK] = make_float4(g.kc[i / NK][i % NK][0], g.kc[i / NK][i % NK][1], g.kc[i / NK][i % NK][2], 0.0f);
-  if (t == 0) {
-    scs.wm1 = g.wm1; scs.hm1 = g.hm1; scs.znear = g.znear; scs.inv_zrange = 1.0f / (g.zfar - g.znear);
-    scs.sp_scale = g.sp_scale; scs.inv2sig2 = g.inv2sig2; scs.inv_wm1 = 1.0f / g.wm1; scs.inv_hm1 = 1.0f / g.hm1;
-    scs.f64 = g.f64; scs.f8 = g.f8; scs.ftex = g.ftex; scs.img = g.img;
-  }
-}
-
-__device__ __forceinline__ void load_weights(uint8_t* dst, const uint8_t* src, uint32_t bytes, uint64_t* wbar) {
-  tc::mbar_expect_tx(wbar, bytes);
-  for (uint32_t off = 0; off < bytes; off += 32768u) {
-    uint32_t n = bytes - off < 32768u ? bytes - off : 32768u;
-    tc::bulk_g2s(dst + off, src + off, n, wbar);
-  }
-  tc::mbar_wait(wbar, 0, 0x30u);
-}
 
 // Colour work list: the entries of the first list whose sample needs a colour (alpha > 0), in list order, as (index into the
 // first list, sample id).  Block-aggregated append (one atomic per 1024 entries).
@@ -197,240 +43,6 @@ colour_list_kernel(const int* __restrict__ list, const int* __restrict__ count_p
       pos += __popc(m[j]);
     }
     __syncthreads();
-  }
-}
-
-// =====================================================================================================================
-// activation tiles, warpgroup synchronisation
-// =====================================================================================================================
-// store N words (packed fp16 pairs) of row r at word columns [c0, c0 + N) of an activation tile; c0 % 4 == 0
-template <int ROWS, int N>
-__device__ __forceinline__ void a_put(uint8_t* tile, int r, int c0, const uint32_t* w) {
-  static_assert(N % 4 == 0, "runs are whole 16-byte chunks");
-#pragma unroll
-  for (int i = 0; i < N; i += 4)
-    *reinterpret_cast<uint4*>(tile + tc::a_word_off<ROWS>(r, c0 + i)) = make_uint4(w[i], w[i + 1], w[i + 2], w[i + 3]);
-}
-__device__ __forceinline__ void a_word(uint8_t* tile64, int r, int c, uint32_t w) {
-  *reinterpret_cast<uint32_t*>(tile64 + tc::a_word_off<64>(r, c)) = w;
-}
-// the activation tile written by this warpgroup's threads becomes visible to its MMAs
-__device__ __forceinline__ void wg_publish(int bar_id) {
-  tc::fence_proxy_async_smem();
-  tc::named_sync(bar_id, 128);
-}
-
-struct Group {   // the 3-view group of this lane: the other two lanes
-  int l1, l2;
-  __device__ explicit Group(int lane) {
-    const int gb = 3 * (lane / 3);
-    l1 = (gb + (lane - gb + 1) % 3) & 31;
-    l2 = (gb + (lane - gb + 2) % 3) & 31;
-  }
-  __device__ float sum(float x) const { return x + __shfl_sync(FULL, x, l1) + __shfl_sync(FULL, x, l2); }
-  __device__ float min3(float x) const { return fminf(x, fminf(__shfl_sync(FULL, x, l1), __shfl_sync(FULL, x, l2))); }
-  __device__ float max3(float x) const { return fmaxf(x, fmaxf(__shfl_sync(FULL, x, l1), __shfl_sync(FULL, x, l2))); }
-};
-
-// =====================================================================================================================
-// geometry front: stages L0-L3 + view pooling.  Warpgroup tile = 64 rows: row warps 0/1 hold rows 0-31 / 32-63 with
-// column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
-// pooling columns, as tc_kmap's runs are laid out).  20 samples per tile.
-// =====================================================================================================================
-constexpr int GWG = 2;                        // warpgroups per CTA (tail kernel; front kernel up to 28 keypoints)
-constexpr int FSPT = 2 * SPW;                 // samples per front tile
-constexpr int D3S = 68;                       // row stride (floats) of the L3 accumulator rows staged for the pooling
-constexpr int POOL_W = 128;                   // pooled [mean 64 | var 64] fp32 per sample
-constexpr long long POOL_SLICE = 1ll << 22;   // samples per front/tail launch pair (bounds the pooled scratch to 2 GiB)
-// activation tile of a front warpgroup: 64 rows of the layer-0 input, which is at least as wide as the 144-wide inputs of
-// L1 / L2 for 9 keypoints and more; fewer keypoints get the L1 / L2 width
-__host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) {
-  return 64u * (uint32_t)(tc_k0p(n_kpt) > 144 ? tc_k0p(n_kpt) : 144) * 2u;
-}
-static_assert(64 * D3S * 4 <= 64 * 144 * 2, "the L3 rows fit in the activation tile they replace");
-// Warpgroups per front CTA: two while the resident W_hi of stages 0..3 and two activation tiles fit in the 227 KB an SM
-// gives a block (up to 28 keypoints: 229 376 B dynamic + the static scene block), one above (29..32 keypoints: K0P 288 / 304)
-constexpr uint32_t SMEM_OPTIN = 227u * 1024u;
-constexpr uint32_t FRONT_STATIC = 2048u;      // static shared memory of the front kernel (SceneS + mbarrier, ptxas)
-static_assert(sizeof(SceneS) + sizeof(uint64_t) <= FRONT_STATIC, "static shared memory of the front kernel");
-__host__ __device__ constexpr uint32_t front_smem_bytes(int n_kpt, int wgs) {
-  return make_tc_plan(n_kpt).st[4].off + (uint32_t)wgs * front_tile_bytes(n_kpt);
-}
-__host__ __device__ constexpr int front_wgs(int n_kpt) { return front_smem_bytes(n_kpt, 2) + FRONT_STATIC <= SMEM_OPTIN ? 2 : 1; }
-static_assert(front_wgs(18) == 2 && front_wgs(24) == 2 && front_wgs(28) == 2 && front_wgs(29) == 1, "front CTA layouts");
-static_assert(front_smem_bytes(KPN_MAX_KPT, 1) + FRONT_STATIC <= SMEM_OPTIN, "one warpgroup fits at the maximum count");
-// offsets of the tail's (4, 5) and the colour head's (6..12) tiles relative to the first of them; the tiles past stage 0 have
-// the same size for every keypoint count, so any count's plan gives them
-constexpr TcPlan REL_PLAN = make_tc_plan(KPN_MAX_KPT);
-
-// one geometry stage of the warpgroup: A (64 rows at `a`) x resident W tile at `b` -> d (N = 128 or 64 fp32 per row)
-template <int N, int KCH>
-__device__ __forceinline__ void front_mma(float* d, const uint8_t* a, uint32_t b, int bar_id) {
-  wg_publish(bar_id);
-  tc::wg_fence();
-  tc::wg_mma<N, KCH>(d, tc::smem_u32(a), 1024u, b, (uint32_t)(N / 8) * 128u, 0u);
-  tc::wg_commit();
-  tc::wg_wait0();
-  tc::named_sync(bar_id, 128);   // every warp's MMAs are complete: the tile may be overwritten
-}
-// softplus epilogue of a 128-wide stage on the fragments: next layer's input words [0, 64); bias_tail: words 60..63 become
-// (1,0),0,0,0 (layer-3 input: bias column + K padding)
-__device__ __forceinline__ void front_epi_sp(const float* d, uint8_t* a, int wq, int lane, bool bias_tail) {
-#pragma unroll
-  for (int m = 0; m < 32; ++m) {
-    const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);
-    uint32_t w = sp_pair(__float_as_uint(d[2 * m]), __float_as_uint(d[2 * m + 1]));
-    if (bias_tail && m >= 30) w = (lane & 3) == 0 ? H2_ONE : 0u;
-    a_word(a, r, c, w);
-  }
-}
-
-// keypoint encodings of pair j (keypoints 2j, 2j+1) as 7 packed fp16 words; the second slot of an odd count's last pair is 0
-template <int NP>
-__device__ __forceinline__ void encode_pair(const SceneS& S, int v, int j, int nk, const float c[3], uint32_t* a) {
-  float e0[7], e1[7];
-  encode_fast(S, v, 2 * j, c, e0);
-  if (j < NP - 1 || 2 * j + 1 < nk) {
-    encode_fast(S, v, 2 * j + 1, c, e1);
-  } else {
-#pragma unroll
-    for (int r = 0; r < 7; ++r) e1[r] = 0.0f;
-  }
-#pragma unroll
-  for (int r = 0; r < 7; ++r) a[r] = tc::pack_h2(e0[r], e1[r]);
-}
-
-// One instantiation per keypoint pair count NP (nk = 2 NP - 1 or 2 NP keypoints).
-template <int NP>
-__global__ void __launch_bounds__(front_wgs(2 * NP) * 128, 1)
-geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __restrict__ wblob, SampleSrc src,
-                 const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
-                 float* __restrict__ pool) {
-  extern __shared__ __align__(1024) uint8_t wsm[];
-  __shared__ uint64_t wbar;
-  __shared__ SceneS scs;
-  constexpr int NK = 2 * NP, FWG = front_wgs(NK);
-  constexpr TcPlan plan = make_tc_plan(NK);
-  constexpr uint32_t WBYTES = plan.st[4].off;        // W_hi of stages 0..3
-  constexpr int PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
-  const long long end = min((long long)*count_ptr, base + len);
-  if (end <= base) return;
-  const int ntiles = (int)((end - base + FSPT - 1) / FSPT);
-  const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31;
-  stage_scene(scs, *scp, nk, t, FWG * 128);
-  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
-  __syncthreads();
-  if (t == 0) load_weights(wsm, wblob, WBYTES, &wbar);
-  __syncthreads();
-  uint8_t* A = wsm + WBYTES + (size_t)wg * front_tile_bytes(NK);
-  float* D3 = reinterpret_cast<float*>(A);
-  const uint32_t W = tc::smem_u32(wsm);
-  const int bar_id = 1 + wg;
-  const int row = (wq & 1) * 32 + lane, h = wq >> 1;
-  const int g = lane / 3, v = lane - 3 * g;           // lanes 30, 31 replay views 0, 1 of the warp's last sample (unused)
-  const Group grp(lane);
-  for (int tile = blockIdx.x * FWG + wg; tile < ntiles; tile += gridDim.x * FWG) {
-    const long long si = base + (long long)tile * FSPT + (wq & 1) * SPW + min(g, SPW - 1);
-    const int id = list[min(si, end - 1)];
-    float p[3], dd[3];
-    fetch_sample(src, id, p, dd);
-    const Proj q = project_s(scs, v, p);
-    const float bw = boundary_weight_fast(q);
-    const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
-    // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap
-    {
-      float c[3];
-      const float* E = scs.E[v];
-      c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
-      c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
-      c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
-      const Taps t64 = make_taps(q.u, q.v, scs.f64.W, scs.f64.H);
-      constexpr int C1 = 7 * PA + FA / 2;             // thread 0's run: words [0, C1); thread 1's: [C1, K0P / 2)
-      static_assert(C1 % 4 == 0 && C1 > 0, "both runs start on a 16-byte chunk");
-      if (h == 0) {
-        uint32_t a[C1];
-#pragma unroll
-        for (int gq = 0; gq < FA / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(scs.f64, v, t64, gq, f);
-          a[7 * PA + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[7 * PA + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
-        }
-#pragma unroll
-        for (int j = 0; j < PA; ++j) encode_pair<NP>(scs, v, j, nk, c, a + 7 * j);
-        a_put<64, C1>(A, row, 0, a);
-      } else {
-        constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
-        constexpr int N1 = tc_k0p(NK) / 2 - C1;
-        static_assert(NE + NF + 1 <= N1, "the bias column is in thread 1's run");
-        uint32_t a[N1];
-#pragma unroll
-        for (int gq = 0; gq < (64 - FA) / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(scs.f64, v, t64, FA / 4 + gq, f);
-          a[NE + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[NE + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
-        }
-#pragma unroll
-        for (int j = PA; j < NP; ++j) encode_pair<NP>(scs, v, j, nk, c, a + 7 * (j - PA));
-        a[NE + NF] = H2_ONE;
-#pragma unroll
-        for (int i = NE + NF + 1; i < N1; ++i) a[i] = 0u;
-        a_put<64, N1>(A, row, C1, a);
-      }
-    }
-    // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720)
-    float d[64];
-    front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
-    front_epi_sp(d, A, wq, lane, false);
-    if (h == 0) {   // layer-1 input: bias chunk
-      const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-      a_put<64, 8>(A, row, 64, b);
-    }
-    front_mma<128, 9>(d, A, W + plan.st[1].off, bar_id);
-    front_epi_sp(d, A, wq, lane, false);
-    if (h == 1) {   // layer-2 input: feat8 | bias chunk
-      uint32_t b[8] = {0u, 0u, 0u, 0u, H2_ONE, 0u, 0u, 0u};
-      const Taps t8 = make_taps(q.u, q.v, scs.f8.W, scs.f8.H);
-      float g8[8];
-      gather_f32<2>(scs.f8, v, t8, 0, g8);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) b[i] = tc::pack_h2(g8[2 * i], g8[2 * i + 1]);
-      a_put<64, 8>(A, row, 64, b);
-    }
-    front_mma<128, 9>(d, A, W + plan.st[2].off, bar_id);
-    front_epi_sp(d, A, wq, lane, true);
-    front_mma<64, 8>(d, A, W + plan.st[3].off, bar_id);
-    // ---- L3 rows to shared memory (over the dead activation tile), then the view pooling: weighted mean || variance over
-    //      the 3 lanes of the group (src/utils.py:722-748); this thread owns 32 of the 64 feature columns
-#pragma unroll
-    for (int m = 0; m < 16; ++m) {
-      const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 8 * (m >> 1) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(D3 + r * D3S + c) = make_float2(d[2 * m], d[2 * m + 1]);
-    }
-    tc::named_sync(bar_id, 128);
-    {
-      const bool writer = lane < 3 * SPW && v == 0 && si < end;
-      float* out = pool + (si - base) * POOL_W + 32 * h;
-      const float* x = D3 + row * D3S + 32 * h;
-#pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4) {
-        const float4 xv = *reinterpret_cast<const float4*>(x + 4 * c4);
-        const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-        float mn[4], vr[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          mn[i] = grp.sum(pw * xs[i]);
-          const float dl = xs[i] - mn[i];
-          vr[i] = grp.sum(pw * dl * dl);
-        }
-        if (writer) {
-          *reinterpret_cast<float4*>(out + 4 * c4) = make_float4(mn[0], mn[1], mn[2], mn[3]);
-          *reinterpret_cast<float4*>(out + 64 + 4 * c4) = make_float4(vr[0], vr[1], vr[2], vr[3]);
-        }
-      }
-    }
-    tc::named_sync(bar_id, 128);   // the L3 rows are read: the next tile's input may overwrite them
   }
 }
 
@@ -573,273 +185,6 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
   }
 }
 
-// =====================================================================================================================
-// colour head.  Warpgroup tile = 128 rows (4 row warps x 10 samples x 3 views); each stage runs as two 64-row MMAs whose
-// accumulators are staged in shared memory (D) for the row threads, which do the cross-view work of the reference.
-// =====================================================================================================================
-constexpr int CWG = 2;                                   // warpgroups per CTA
-constexpr int CDS = 68;                                  // row stride (floats) of the staged accumulators
-constexpr uint32_t CA_BYTES = 128 * 112 * 2;             // activation tile (widest colour input: BASE0, K = 112)
-constexpr uint32_t CD_BYTES = 128 * CDS * 4;
-
-struct ColCtx {
-  uint8_t* A;
-  float* D;
-  uint32_t wbase;   // shared address of the colour stages' weights (plan offset of stage 6 at 0)
-  int bar_id, row, wq, lane;
-  Group grp;
-};
-
-template <int STAGE>
-__device__ __forceinline__ void col_mma(const ColCtx& c) {
-  constexpr TcPlan plan = REL_PLAN;
-  constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
-  const uint32_t b = c.wbase + (plan.st[STAGE].off - plan.st[GEO_NSTAGE].off);
-  wg_publish(c.bar_id);
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    float d[Np / 2];
-    tc::wg_fence();
-    tc::wg_mma<Np, Kp / 16>(d, tc::smem_u32(c.A) + 1024u * (uint32_t)half, 2048u, b, (uint32_t)(Np / 8) * 128u, 0u);
-    tc::wg_commit();
-    tc::wg_wait0();
-#pragma unroll
-    for (int m = 0; m < Np / 4; ++m) {
-      const int r = 64 * half + 16 * c.wq + (c.lane >> 2) + 8 * (m & 1), col = 8 * (m >> 1) + 2 * (c.lane & 3);
-      *reinterpret_cast<float2*>(c.D + r * CDS + col) = make_float2(d[2 * m], d[2 * m + 1]);
-    }
-  }
-  tc::named_sync(c.bar_id, 128);   // accumulators staged, every MMA has read the activation tile
-}
-template <int N>
-__device__ __forceinline__ void d_get(const ColCtx& c, int c0, float* x) {
-#pragma unroll
-  for (int i = 0; i < N; i += 4) {
-    const float4 f = *reinterpret_cast<const float4*>(c.D + c.row * CDS + c0 + i);
-    x[i] = f.x; x[i + 1] = f.y; x[i + 2] = f.z; x[i + 3] = f.w;
-  }
-}
-// staged accumulator columns [0, 32*NCH) -> act(acc + bias) as the next input's words [0, 16*NCH)
-template <int NCH, int ACT>  // ACT 1 = softplus100, 2 = ELU
-__device__ __forceinline__ void col_epi(const ColCtx& c, const float* __restrict__ bias) {
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    float x[32];
-    d_get<32>(c, 32 * ch, x);
-    uint32_t o[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float x0 = x[2 * i] + bias[ch * 32 + 2 * i], x1 = x[2 * i + 1] + bias[ch * 32 + 2 * i + 1];
-      if (ACT == 1) { x0 = sp_fast(x0); x1 = sp_fast(x1); }
-      else { x0 = elu_fast(x0); x1 = elu_fast(x1); }
-      o[i] = tc::pack_h2(x0, x1);
-    }
-    a_put<128, 16>(c.A, c.row, 16 * ch, o);
-  }
-}
-
-// Colour pass for one tile of the second work list (entries: x = slot of the latent in the scratch buffer, y = sample id).
-__device__ __forceinline__ void color_tile(const SceneS& sc, const TcConsts& C, const SampleSrc& src,
-                                           const int2* __restrict__ list2, const int* __restrict__ list1, int count, int tile,
-                                           const ColCtx& cx, const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
-  const int lane = cx.lane;
-  const int g = lane / 3;
-  const int v = lane - 3 * g;
-  const int si = tile * SPT + cx.wq * SPW + min(g, SPW - 1);
-  const bool writer = (lane < 3 * SPW) && (v == 0) && (si < count);
-  // entry: x = index into the first work list (where the latent sits and, + list_base, where the colour goes), y = sample id;
-  // query mode shades every valid sample: the first list itself is the work list
-  const int e = min(si, count - 1);
-  const int2 ent = list2 ? list2[e] : make_int2(e, list1[e]);
-  const int id = ent.y;
-  float p[3], d[3];
-  fetch_sample(src, id, p, d);
-  const Proj q = project_s(sc, v, p);
-  float lat[24];
-  {
-    uint4 w[3];
-    w[0] = __ldg(lat_in + 3ll * ent.x + 0); w[1] = __ldg(lat_in + 3ll * ent.x + 1); w[2] = __ldg(lat_in + 3ll * ent.x + 2);
-    const __half2* hp = reinterpret_cast<const __half2*>(w);
-#pragma unroll
-    for (int i = 0; i < 12; ++i) { float2 t2 = __half22float2(hp[i]); lat[2 * i] = t2.x; lat[2 * i + 1] = t2.y; }
-  }
-  // ---- colour branch inputs (src/model.py:806-832)
-  float rgb[3], f[35], rd[4];
-  {
-    const Taps ti = make_taps(q.u, q.v, sc.img.W, sc.img.H);
-    float c4[4];
-    gather_f32<1>(sc.img, v, ti, 0, c4);
-    rgb[0] = c4[0]; rgb[1] = c4[1]; rgb[2] = c4[2];
-    f[0] = c4[0]; f[1] = c4[1]; f[2] = c4[2];
-    const Taps tt = make_taps(q.u, q.v, sc.ftex.W, sc.ftex.H);
-    float t8[8];
-    gather_f32<2>(sc.ftex, v, tt, 0, t8);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[3 + i] = t8[i];
-#pragma unroll
-    for (int i = 0; i < 24; ++i) f[11 + i] = lat[i];
-    {  // [unit(dir - dir_src), dir . dir_src], reference src/model.py:825-832
-      float r[3] = {p[0] - sc.C[v][0], p[1] - sc.C[v][1], p[2] - sc.C[v][2]};
-      float n = fmaxf(sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2]), 1e-12f);
-      r[0] /= n; r[1] /= n; r[2] /= n;
-      float e[3] = {d[0] - r[0], d[1] - r[1], d[2] - r[2]};
-      float en = fmaxf(sqrtf(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), 1e-6f);
-      rd[0] = e[0] / en; rd[1] = e[1] / en; rd[2] = e[2] / en;
-      rd[3] = r[0] * d[0] + r[1] * d[1] + r[2] * d[2];
-    }
-  }
-  {  // ray-direction encoder 4->16->35, ELU, added onto the features (src/model.py:1279-1284): first layer in fp32 on the CUDA
-     // cores, second layer (stage 12, bias as K row 16) on the tensor core
-    uint32_t a[16];
-#pragma unroll
-    for (int o = 0; o < 16; o += 2) {
-      float acc0 = C.b_re0[o], acc1 = C.b_re0[o + 1];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { acc0 = fmaf(C.w_re0[o][i], rd[i], acc0); acc1 = fmaf(C.w_re0[o + 1][i], rd[i], acc1); }
-      a[o / 2] = tc::pack_h2(elu_fast(acc0), elu_fast(acc1));
-    }
-    a[8] = H2_ONE;   // bias column
-#pragma unroll
-    for (int i = 9; i < 16; ++i) a[i] = 0u;
-    a_put<128, 16>(cx.A, cx.row, 0, a);
-    col_mma<12>(cx);
-    float r[36];
-    d_get<36>(cx, 0, r);
-#pragma unroll
-    for (int o = 0; o < 35; ++o) f[o] += elu_fast(r[o]);
-  }
-  float om;  // blending weight (src/model.py:1286-1289), mask == 1
-  {
-    float ex = ex2f(C.ani_abs * LOG2E * (rd[3] - 1.0f));
-    float e = ex - cx.grp.min3(ex);
-    om = e / (cx.grp.sum(e) + 1e-8f);
-  }
-  {  // BASE0 input [mean35 | var35 | f35 | 0-pad] (src/model.py:1291-1292)
-    float mean[35], var[35];
-#pragma unroll
-    for (int c = 0; c < 35; ++c) {
-      mean[c] = cx.grp.sum(om * f[c]);
-      float dl = f[c] - mean[c];
-      var[c] = cx.grp.sum(om * dl * dl);
-    }
-    uint32_t a[56];
-#pragma unroll
-    for (int j = 0; j < 56; ++j) {
-      const int e0 = 2 * j, e1 = 2 * j + 1;
-      float x0 = e0 < 35 ? mean[e0 < 35 ? e0 : 0] : e0 < 70 ? var[e0 < 70 ? (e0 >= 35 ? e0 - 35 : 0) : 0]
-                 : e0 < 105 ? f[e0 >= 70 ? (e0 < 105 ? e0 - 70 : 0) : 0] : 0.0f;
-      float x1 = e1 < 35 ? mean[e1 < 35 ? e1 : 0] : e1 < 70 ? var[e1 < 70 ? (e1 >= 35 ? e1 - 35 : 0) : 0]
-                 : e1 < 105 ? f[e1 >= 70 ? (e1 < 105 ? e1 - 70 : 0) : 0] : 0.0f;
-      a[j] = tc::pack_h2(x0, x1);
-    }
-    a_put<128, 56>(cx.A, cx.row, 0, a);
-  }
-  col_mma<6>(cx);
-  // ---- BASE0 -> BASE1
-  col_epi<2, 2>(cx, C.b_base0);
-  col_mma<7>(cx);
-  float x[32];
-  {
-    float r[32];
-    d_get<32>(cx, 0, r);
-    uint32_t o[16];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) x[i] = elu_fast(r[i] + C.b_base1[i]);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * om, x[2 * i + 1] * om);  // vis_layer1(x * weight)
-    a_put<128, 16>(cx.A, cx.row, 0, o);
-  }
-  col_mma<8>(cx);
-  // ---- VIS1A -> VIS1B (src/model.py:1294-1296)
-  col_epi<1, 2>(cx, C.b_vis1a);
-  col_mma<9>(cx);
-  {
-    float r[36];
-    d_get<36>(cx, 0, r);
-    float sg = sig_fast(elu_fast(r[32] + C.b_vis1b[32]));
-    uint32_t o[16];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) x[i] += elu_fast(r[i] + C.b_vis1b[i]);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * sg, x[2 * i + 1] * sg);  // x * sigmoid(vis) * mask
-    a_put<128, 16>(cx.A, cx.row, 0, o);
-  }
-  col_mma<10>(cx);
-  // ---- VIS2A (+ 32->1 sigmoid on CUDA cores) -> OUT0 input [x32 | vis | ray_diff4 | 0-pad] (src/model.py:1297-1300)
-  {
-    float r[32];
-    d_get<32>(cx, 0, r);
-    float dot = C.b_vis2b;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) dot = fmaf(C.w_vis2b[i], elu_fast(r[i] + C.b_vis2a[i]), dot);
-    float vis2 = sig_fast(dot);
-    uint32_t o[24];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i], x[2 * i + 1]);
-    o[16] = tc::pack_h2(vis2, rd[0]);
-    o[17] = tc::pack_h2(rd[1], rd[2]);
-    o[18] = tc::pack_h2(rd[3], 0.0f);
-#pragma unroll
-    for (int i = 19; i < 24; ++i) o[i] = 0u;
-    a_put<128, 24>(cx.A, cx.row, 0, o);
-  }
-  col_mma<11>(cx);
-  // ---- OUT0 -> 16->8->1 on CUDA cores -> softmax over the views -> blended colour (src/model.py:1300-1301)
-  float logit;
-  {
-    float r[16];
-    d_get<16>(cx, 0, r);
-    float h16[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) h16[i] = elu_fast(r[i] + C.b_out0[i]);
-    logit = C.b_out2;
-#pragma unroll
-    for (int o = 0; o < 8; ++o) {
-      float acc = C.b_out1[o];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc = fmaf(C.w_out1[o][i], h16[i], acc);
-      logit = fmaf(C.w_out2[o], elu_fast(acc), logit);
-    }
-  }
-  {
-    float e = ex2f((logit - cx.grp.max3(logit)) * LOG2E);
-    float inv = 1.0f / cx.grp.sum(e);
-    float r0 = cx.grp.sum(e * rgb[0]) * inv, r1 = cx.grp.sum(e * rgb[1]) * inv, r2 = cx.grp.sum(e * rgb[2]) * inv;
-    if (writer) {
-      float* o = query_mode ? so.out5 + 5ll * id + 2 : so.rgb + 3ll * (so.list_base + ent.x);
-      o[0] = r0; o[1] = r1; o[2] = r2;
-    }
-  }
-}
-
-// wcol: the blob's tile of stage 6 (the colour stages' tiles follow it)
-__global__ void __launch_bounds__(CWG * 128, 1)
-shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcConsts C, const uint8_t* __restrict__ wcol,
-                   SampleSrc src, const int2* __restrict__ list2, const int* __restrict__ list1,
-                   const int* __restrict__ count_ptr, const uint4* __restrict__ lat_in, int query_mode, ShadeOut so) {
-  extern __shared__ __align__(1024) uint8_t wsm[];
-  __shared__ uint64_t wbar;
-  __shared__ SceneS scs;
-  constexpr TcPlan plan = REL_PLAN;
-  constexpr uint32_t WBYTES = plan.total_bytes - plan.st[GEO_NSTAGE].off;
-  constexpr uint32_t WPAD = (WBYTES + 1023u) / 1024u * 1024u;
-  const int t = threadIdx.x, wg = t >> 7;
-  const int count = *count_ptr;
-  const int ntiles = (count + SPT - 1) / SPT;
-  if (blockIdx.x * CWG >= ntiles) return;
-  stage_scene(scs, *scp, 0, t, CWG * 128);   // the colour head reads no keypoints
-  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
-  __syncthreads();
-  if (t == 0) load_weights(wsm, wcol, WBYTES, &wbar);   // the colour stages' weight tiles, once per CTA
-  __syncthreads();
-  const int lane = t & 31;
-  ColCtx cx{wsm + WPAD + (size_t)wg * (CA_BYTES + CD_BYTES), nullptr, tc::smem_u32(wsm), 1 + wg, t & 127, (t >> 5) & 3, lane,
-            Group(lane)};
-  cx.D = reinterpret_cast<float*>(cx.A + CA_BYTES);
-  for (int tile = blockIdx.x * CWG + wg; tile < ntiles; tile += gridDim.x * CWG)
-    color_tile(scs, C, src, list2, list1, count, tile, cx, lat_in, query_mode, so);
-}
-
 }  // namespace
 
 size_t tc_weight_blob_bytes(int n_kpt) { return make_tc_plan(n_kpt).total_bytes; }
@@ -849,111 +194,83 @@ size_t tc_weight_lo_bytes(int n_kpt) {
 }
 size_t tc_pool_bytes(long long n_max) { return (size_t)(n_max < POOL_SLICE ? n_max : POOL_SLICE) * POOL_W * sizeof(float); }
 bool tc_supported(int n_views, int n_kpt, int sp_level) {
-  return n_views == 3 && n_kpt >= 1 && n_kpt <= KPN_MAX_KPT && sp_level == 3;
+  return (n_views == 3 || n_views == 4) && n_kpt >= 1 && n_kpt <= KPN_MAX_KPT && sp_level == 3;
 }
 
-template <int NP>
-static cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo,
-                                  int lo_mask, const SampleSrc& src, const int* list, const int* counter, long long n_max,
-                                  int query_mode, const ShadeOut& so, uint4* lat, float* pool, int2* list2, int* count2, int num_sms,
-                                  cudaEvent_t after_geo, int* launches, cudaStream_t st) {
-  constexpr int NK = 2 * NP, FWG = front_wgs(NK);
-  constexpr TcPlan plan = make_tc_plan(NK);
-  const size_t smem_front = front_smem_bytes(NK, FWG);
+cudaError_t launch_geo_tail(const TcConsts& C, const uint8_t* wtail, const uint8_t* wlo, int lo_mask, const int* list,
+                            const int* counter, long long base, long long len, const float* pool, int query_mode, const ShadeOut& so,
+                            uint4* lat, int num_sms, cudaStream_t st) {
   constexpr TcPlan rel = REL_PLAN;
   constexpr uint32_t smem_tail = 2 * (rel.st[GEO_NSTAGE].off - rel.st[4].off) + GWG * TAIL_TILE_BYTES;
-  constexpr uint32_t smem_col = (rel.total_bytes - rel.st[GEO_NSTAGE].off + 1023) / 1024 * 1024 + CWG * (CA_BYTES + CD_BYTES);
   static std::atomic<bool> attr[64];   // function attributes are per device (zero-initialised; setting them twice is harmless)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
-    if (e != cudaSuccess) return e;
-    // the tail and colour kernels serve every keypoint count
-    e = cudaFuncSetAttribute(geo_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(shade_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_col);
+    cudaError_t e = cudaFuncSetAttribute(geo_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
-  const uint8_t* wtail = wblob + plan.st[4].off;
-  const uint8_t* wcol = wblob + plan.st[GEO_NSTAGE].off;
-  auto grid_for = [&](long long tiles, int per_cta) {
-    const long long g = (tiles + per_cta - 1) / per_cta;
-    return (int)(g < 1 ? 1 : (g > num_sms ? num_sms : g));
-  };
-  cudaError_t e = cudaSuccess;
-  // the device-side count is not known here: every slice of [0, n_max) is launched, slices past the count exit at once
-  const long long nslices = n_max > POOL_SLICE ? (n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
-  for (long long s = 0; s < nslices; ++s) {
-    const long long base = s * POOL_SLICE, len = n_max - base < POOL_SLICE ? n_max - base : POOL_SLICE;
-    geo_front_kernel<NP><<<grid_for((len + FSPT - 1) / FSPT, FWG), FWG * 128, smem_front, st>>>(sc, nk, wblob, src, list, counter,
-                                                                                                  base, len, pool);
-    geo_tail_kernel<<<grid_for((len + 63) / 64, GWG), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len,
-                                                                                   pool, query_mode, so, lat);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    *launches += 2;
-  }
-  if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
-  const int grid = grid_for((n_max + SPT - 1) / SPT, CWG);
-  if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
-    shade_color_kernel<<<grid, CWG * 128, smem_col, st>>>(sc, C, wcol, src, nullptr, list, counter, lat, query_mode, so);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    *launches += 1;
-    return cudaMemcpyAsync(count2, counter, sizeof(int), cudaMemcpyDeviceToDevice, st);   // statistics: every valid sample was coloured
-  }
-  const long long lb = (n_max + 1023) / 1024;
-  colour_list_kernel<<<(int)(lb < 1 ? 1 : (lb > num_sms * 8 ? num_sms * 8 : lb)), 256, 0, st>>>(list, counter, so.ao, so.list_base,
-                                                                                                 list2, count2);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  shade_color_kernel<<<grid, CWG * 128, smem_col, st>>>(sc, C, wcol, src, list2, nullptr, count2, lat, query_mode, so);
-  *launches += 2;
+  geo_tail_kernel<<<tc_grid((len + 63) / 64, GWG, num_sms), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len,
+                                                                                       pool, query_mode, so, lat);
   return cudaGetLastError();
 }
 
-using LaunchTc = decltype(&launch_tc_impl<1>);
-template <int... I>
-static constexpr std::array<LaunchTc, sizeof...(I)> launch_table(std::integer_sequence<int, I...>) {
-  return {&launch_tc_impl<I + 1>...};
+cudaError_t launch_colour_list(const int* list, const int* counter, const float2* ao, int list_base, int2* list2, int* count2,
+                               long long n_max, int num_sms, cudaStream_t st) {
+  const long long lb = (n_max + 1023) / 1024;
+  colour_list_kernel<<<(int)(lb < 1 ? 1 : (lb > num_sms * 8 ? num_sms * 8 : lb)), 256, 0, st>>>(list, counter, ao, list_base, list2,
+                                                                                                 count2);
+  return cudaGetLastError();
 }
-// launch_tc_impl<NP> for NP = 1 .. KPN_MAX_KPT / 2 keypoint pairs
-static constexpr std::array<LaunchTc, KPN_MAX_KPT / 2> LAUNCH_TC = launch_table(std::make_integer_sequence<int, KPN_MAX_KPT / 2>{});
 
-cudaError_t launch_shade_tc(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term, int n_kpt,
-                            const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
+cudaError_t launch_shade_tc(const DevScene* sc, int n_views, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term,
+                            int n_kpt, const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
                             const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
                             cudaEvent_t after_geo, int* launches, cudaStream_t st) {
   // W_lo and A_lo passes of the density tail (stages 4, 5: bits 4, 5 and 6, 7); single-term weights keep the A_lo passes
   const int lo_mask = two_term ? 0xF0 : 0xC0;
-  if (n_kpt < 1 || n_kpt > KPN_MAX_KPT) return cudaErrorInvalidValue;
-  return LAUNCH_TC[tc_npair(n_kpt) - 1](sc, n_kpt, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so,
-                                        (uint4*)lat_scratch, (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo,
-                                        launches, st);
+  if (n_views == 3)
+    return launch_tc_views<3>(sc, C, wblob, wlo, lo_mask, n_kpt, src, list, counter, n_max, query_mode, so, lat_scratch, pool_scratch,
+                              list2, count2, num_sms, after_geo, launches, st);
+  if (n_views == 4)
+    return launch_shade_tc_v4(sc, C, wblob, wlo, lo_mask, n_kpt, src, list, counter, n_max, query_mode, so, lat_scratch, pool_scratch,
+                              list2, count2, num_sms, after_geo, launches, st);
+  return cudaErrorInvalidValue;
 }
 
-// Watchdog state of this module's kernels: out[0] != 0 -> some barrier wait gave up at block out[1], thread out[2], tag out[3].
+// Watchdog state of the tensor-core kernels.  Every translation unit has its own copy of the words (kpn_tc.cuh): the 3-view
+// module's (with the shared tail kernel) and the 4-view module's; out[0] != 0 -> some barrier wait gave up at block out[1],
+// thread out[2], tag out[3].
+static_assert(TC_WD_MODULES == 2, "the 3-view and the 4-view module");
+static cudaError_t wd_words(void* w[TC_WD_MODULES]) {
+  cudaError_t e = cudaGetSymbolAddress(&w[0], tc::kpn_wd);
+  return e != cudaSuccess ? e : tc_watchdog_addr_v4(&w[1]);
+}
 cudaError_t tc_watchdog_read(unsigned int out[8], bool reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out, tc::kpn_wd, 8 * sizeof(unsigned int));
-  if (e == cudaSuccess && reset) {
-    const unsigned int z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    e = cudaMemcpyToSymbol(tc::kpn_wd, z, sizeof(z));
-  }
+  void* w[TC_WD_MODULES];
+  unsigned int both[TC_WD_MODULES * TC_WD_WORDS];
+  cudaError_t e = wd_words(w);
+  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m) e = cudaMemcpy(both + TC_WD_WORDS * m, w[m], TC_WD_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return e;
+  const unsigned int* first = both[0] != 0u || both[TC_WD_WORDS] == 0u ? both : both + TC_WD_WORDS;
+  for (int i = 0; i < 8; ++i) out[i] = first[i];
+  for (int m = 0; m < TC_WD_MODULES && reset && e == cudaSuccess; ++m) e = cudaMemset(w[m], 0, TC_WD_WORDS * sizeof(unsigned int));
   return e;
 }
 
-cudaError_t tc_watchdog_read_async(unsigned int* pinned_out8, cudaStream_t st) {
-  return cudaMemcpyFromSymbolAsync(pinned_out8, tc::kpn_wd, 8 * sizeof(unsigned int), 0, cudaMemcpyDeviceToHost, st);
+cudaError_t tc_watchdog_read_async(unsigned int* pinned_out, cudaStream_t st) {
+  void* w[TC_WD_MODULES];
+  cudaError_t e = wd_words(w);
+  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m)
+    e = cudaMemcpyAsync(pinned_out + TC_WD_WORDS * m, w[m], TC_WD_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
+  return e;
 }
 cudaError_t tc_watchdog_clear_async(cudaStream_t st) {
-  void* p = nullptr;
-  cudaError_t e = cudaGetSymbolAddress(&p, tc::kpn_wd);
-  if (e != cudaSuccess) return e;
-  return cudaMemsetAsync(p, 0, 8 * sizeof(unsigned int), st);
+  void* w[TC_WD_MODULES];
+  cudaError_t e = wd_words(w);
+  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m) e = cudaMemsetAsync(w[m], 0, TC_WD_WORDS * sizeof(unsigned int), st);
+  return e;
 }
-
 // stage-timing instrumentation is not built for this architecture's kernels
 cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles) {
   (void)out; (void)n_words; (void)n_tiles;

@@ -96,7 +96,7 @@ def silhouette_masks(K: np.ndarray, extrin: np.ndarray, src_size: int, semi_axes
 
 
 def make_scene(src_size: int = 512, n_views: int = 3, n_kpt: int = 18, seed: int = 2,
-               src_azimuths=(0.0, 2.1, 4.2), fg_hole: bool = False, fg_mode: str | None = None,
+               src_azimuths=(0.0, 2.1, 4.2, 5.25), fg_hole: bool = False, fg_mode: str | None = None,
                src_height: int | None = None) -> dict:
     """Source-side inputs of the hot path (everything ``query`` reads, reference ``src/model.py:690-782``).
 
