@@ -233,7 +233,7 @@ struct Group<3> {
 // column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
 // pooling columns, as tc_kmap's runs are laid out).  2 * spw(NV) samples per tile: 20 with 3 views, 16 with 4.
 // =====================================================================================================================
-constexpr int GWG = 2;                        // warpgroups per CTA (tail kernel; front kernel up to 28 keypoints)
+constexpr int GWG = 2;                        // warpgroups per CTA of the tail kernel (the front kernel's: front_wgs)
 __host__ __device__ constexpr int fspt(int nv) { return 2 * spw(nv); }   // samples per front tile
 constexpr int D3S = 68;                       // row stride (floats) of the L3 accumulator rows staged for the pooling
 constexpr int POOL_W = 128;                   // pooled [mean 64 | var 64] fp32 per sample
@@ -244,8 +244,13 @@ __host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) {
   return 64u * (uint32_t)(tc_k0p(n_kpt) > 144 ? tc_k0p(n_kpt) : 144) * 2u;
 }
 static_assert(64 * D3S * 4 <= 64 * 144 * 2, "the L3 rows fit in the activation tile they replace");
-// Warpgroups per front CTA: two while the resident W_hi of stages 0..3 and two activation tiles fit in the 227 KB an SM
-// gives a block (up to 28 keypoints: 229 376 B dynamic + the static scene block), one above (29..32 keypoints: K0P 288 / 304)
+// Warpgroups per front CTA: as many tiles as fit beside the resident W_hi of stages 0..3 in the 227 KB an SM gives a block,
+// up to three.  The row threads' gathers are latency bound, so a third warpgroup helps hide them; the register file caps the
+// CTA at three (168 registers per thread at 384 threads).  Three tiles fit up to K0P 208 (20 keypoints: 223 232 B dynamic +
+// the static scene block), two up to 28 keypoints (229 376 B), one above (29..32 keypoints: K0P 288 / 304).
+// Three warpgroups also need K0P >= 192 (15..20 keypoints): with narrower layer-0 inputs the split puts up to all 64 feat64
+// channels (64 LDG.128 taps) on one thread of a row, and built for 168 registers ptxas spills or serialises the wgmma chain of some
+// of those pair counts (NP 1, 2, 4 with 3 views; 4, 7 with 4 views), so 1..14 keypoints keep two.
 constexpr uint32_t SMEM_OPTIN = 227u * 1024u;
 // static shared memory of the front kernel (SceneS<NV> + mbarrier, ptxas): 2 000 B with 3 views, 2 624 B with 4
 constexpr uint32_t FRONT_STATIC_V3 = 2048u;
@@ -257,11 +262,17 @@ __host__ __device__ constexpr uint32_t front_smem_bytes(int n_kpt, int wgs) {
   return make_tc_plan(n_kpt).st[4].off + (uint32_t)wgs * front_tile_bytes(n_kpt);
 }
 __host__ __device__ constexpr int front_wgs(int n_kpt, int nv) {
-  return front_smem_bytes(n_kpt, 2) + front_static(nv) <= SMEM_OPTIN ? 2 : 1;
+  return tc_k0p(n_kpt) >= 192 && front_smem_bytes(n_kpt, 3) + front_static(nv) <= SMEM_OPTIN ? 3
+         : front_smem_bytes(n_kpt, 2) + front_static(nv) <= SMEM_OPTIN                       ? 2
+                                                                                              : 1;
 }
-static_assert(front_wgs(18, 3) == 2 && front_wgs(24, 3) == 2 && front_wgs(28, 3) == 2 && front_wgs(29, 3) == 1, "front CTA layouts");
-static_assert(front_wgs(18, 4) == 2 && front_wgs(24, 4) == 2 && front_wgs(28, 4) == 2 && front_wgs(29, 4) == 1,
-              "4-view front CTA layouts: the larger scene block keeps two warpgroups up to 28 keypoints");
+static_assert(front_wgs(1, 3) == 2 && front_wgs(14, 3) == 2 && front_wgs(15, 3) == 3 && front_wgs(18, 3) == 3 &&
+                  front_wgs(20, 3) == 3 && front_wgs(21, 3) == 2 && front_wgs(24, 3) == 2 && front_wgs(28, 3) == 2 &&
+                  front_wgs(29, 3) == 1, "front CTA layouts");
+static_assert(front_wgs(1, 4) == 2 && front_wgs(14, 4) == 2 && front_wgs(15, 4) == 3 && front_wgs(18, 4) == 3 &&
+                  front_wgs(20, 4) == 3 && front_wgs(21, 4) == 2 && front_wgs(24, 4) == 2 && front_wgs(28, 4) == 2 &&
+                  front_wgs(29, 4) == 1,
+              "4-view front CTA layouts: the larger scene block keeps three warpgroups up to 20 keypoints, two up to 28");
 static_assert(front_smem_bytes(KPN_MAX_KPT, 1) + FRONT_STATIC_V4 <= SMEM_OPTIN, "one warpgroup fits at the maximum count");
 // offsets of the tail's (4, 5) and the colour head's (6..12) tiles relative to the first of them; the tiles past stage 0 have
 // the same size for every keypoint count, so any count's plan gives them
@@ -443,7 +454,7 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
 // colour head.  Warpgroup tile = 128 rows (4 row warps x spw(NV) samples x NV views: 40 samples with 3 views, 32 with 4; each
 // stage runs as two 64-row MMAs whose accumulators are staged in shared memory (D) for the row threads, which do the cross-view work of the reference.
 // =====================================================================================================================
-constexpr int CWG = 2;                                   // warpgroups per CTA
+constexpr int CWG = 3;                                   // warpgroups per CTA (168 registers per thread)
 constexpr int CDS = 68;                                  // row stride (floats) of the staged accumulators
 constexpr uint32_t CA_BYTES = 128 * 112 * 2;             // activation tile (widest colour input: BASE0, K = 112)
 constexpr uint32_t CD_BYTES = 128 * CDS * 4;
