@@ -162,10 +162,14 @@ void kpn_destroy(kpn_ctx* ctx);
 const char* kpn_last_error(const kpn_ctx* ctx);
 
 /* Folds weight norm, transposes/pads and uploads the hot-path parameters.
- * Stands in for load_state_dict on mlp_geo / mlp_tex / ibr_compress_gfeat (reference src/model.py:113-117). */
+ * Stands in for load_state_dict on mlp_geo / mlp_tex / ibr_compress_gfeat (reference src/model.py:113-117).
+ * With a scene bound, new weights with the same n_kpt keep it bound and rewrite its encoding constants (sp_level,
+ * sp_scale, sp_sigma), so the next render equals one after a fresh kpn_set_scene; a different n_kpt unbinds it, and
+ * kpn_render / kpn_query return KPN_ERR_STATE until kpn_set_scene is called again. */
 int kpn_set_weights(kpn_ctx* ctx, const kpn_weights* w);
 
-/* Re-layouts the source feature maps into channel-last atlases and derives per-view constants.
+/* Re-layouts the source feature maps into channel-last atlases and derives per-view constants.  The keypoint-encoding
+ * constants come from the weights set last (see kpn_set_weights).
  * Stands in for attach_im_feat / the feat_geo, feat_tex, cam_in, sp_data arguments (reference src/model.py:642-680,922). */
 int kpn_set_scene(kpn_ctx* ctx, const kpn_scene* scene, void* stream);
 

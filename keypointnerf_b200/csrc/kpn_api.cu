@@ -191,6 +191,15 @@ static void expected_dims(int n_kpt, int sp_level, int dims[NLAYER][2]) {
   memcpy(dims, t, sizeof(t));
 }
 
+// The keypoint-encoding constants of the scene block (sp_scale .. freq), from the weights' sp_args.
+static void set_encoding(const kpn_ctx* c, DevScene& h) {
+  h.sp_scale = c->sp_scale;
+  h.inv2sig2 = 1.0f / (2.0f * c->sp_sigma * c->sp_sigma);
+  h.sp_level = c->sp_level;
+  double val = 1.0;
+  for (int l = 0; l < MAX_SPL; ++l) { h.freq[l] = l < c->sp_level ? (float)(3.14159265358979323846 * val) : 0.0f; val *= 2.0; }
+}
+
 extern "C" int kpn_set_weights(kpn_ctx* c, const kpn_weights* w) {
   if (!c || !w) return KPN_ERR_ARG;
   DeviceGuard g(c->device);
@@ -286,8 +295,22 @@ extern "C" int kpn_set_weights(kpn_ctx* c, const kpn_weights* w) {
     T.ani_abs = std::fabs(w->ani_al);
     c->tc_weights = true;
   }
+  const bool same_kpt = c->n_kpt == w->n_kpt;
   c->n_kpt = w->n_kpt; c->sp_level = w->sp_level; c->sp_scale = w->sp_scale; c->sp_sigma = w->sp_sigma;
   c->have_weights = true;
+  // A bound scene carries the encoding constants of the weights it was bound with: rewrite them, so that the next render uses
+  // the new sp_level / scale / sigma (the device is idle, see above).  Its keypoints can not serve another count: unbind it.
+  if (c->have_scene) {
+    if (!same_kpt) {
+      c->have_scene = false;
+    } else {
+      DevScene h;
+      set_encoding(c, h);
+      const size_t lo = offsetof(DevScene, sp_scale), hi = offsetof(DevScene, freq) + sizeof(h.freq);
+      KPN_CUDA(c, cudaMemcpy(reinterpret_cast<char*>(c->d_scene) + lo, reinterpret_cast<const char*>(&h) + lo, hi - lo,
+                             cudaMemcpyHostToDevice));
+    }
+  }
   return KPN_OK;
 }
 
@@ -320,13 +343,7 @@ extern "C" int kpn_set_scene(kpn_ctx* c, const kpn_scene* s, void* stream) {
   h.znear = s->znear; h.zfar = s->zfar;
   h.sdf_invalid = 0.1f / s->nml_scale;
   h.use_fg = s->fg != nullptr;
-  h.sp_scale = c->sp_scale;
-  h.inv2sig2 = 1.0f / (2.0f * c->sp_sigma * c->sp_sigma);
-  h.sp_level = c->sp_level;
-  {
-    double val = 1.0;
-    for (int l = 0; l < c->sp_level; ++l) { h.freq[l] = (float)(3.14159265358979323846 * val); val *= 2.0; }
-  }
+  set_encoding(c, h);
   struct MapIn { const float* src; int C, H, W, Cp; } maps[4] = {
       {s->feat64, s->f64_c, s->f64_h, s->f64_w, 64}, {s->feat8, s->f8_c, s->f8_h, s->f8_w, 8},
       {s->feat_tex, s->ftex_c, s->ftex_h, s->ftex_w, 8}, {s->img, 3, s->img_h, s->img_w, 4}};

@@ -155,9 +155,10 @@ def make_target(size: int = 512, azimuth: float = 1.0, znear: float = 2.0, zfar:
             "znear": znear, "zfar": zfar, "nml_scale": 100.0}
 
 
-def layer_table(n_kpt: int = 18):
-    """(key prefix, out, in, weight-normed?) for every dense layer on the path (SURVEY.md Appendix D)."""
-    enc = 7 * n_kpt
+def layer_table(n_kpt: int = 18, sp_level: int = 3):
+    """(key prefix, out, in, weight-normed?) for every dense layer on the path (SURVEY.md Appendix D).  Layer 0 reads the
+    (1 + 2 sp_level) n_kpt keypoint encoding and the 64 feat64 channels."""
+    enc = (1 + 2 * sp_level) * n_kpt
     return [
         ("mlp_geo.layers1.layers.0.linear", 128, enc + 64, True),
         ("mlp_geo.layers1.layers.1.linear", 128, 128, True),
@@ -181,13 +182,19 @@ def layer_table(n_kpt: int = 18):
     ]
 
 
-def make_weights(n_kpt: int = 18, seed: int = 26, density_gain: float = 30.0) -> dict:
-    """Seeded hot-path parameters keyed like the reference state_dict."""
+def make_weights(n_kpt: int = 18, seed: int = 26, density_gain: float = 30.0, sp_level: int = 3, dz_scale: float = 1.0) -> dict:
+    """Seeded hot-path parameters keyed like the reference state_dict, for a ``sp_level`` keypoint encoding.
+
+    ``dz_scale``: the layer-0 columns that read the encoding's dz row (the first n_kpt inputs) are divided by it, so that with
+    ``sp_args.scale = dz_scale`` layer 0 sees inputs of the size a model trained in those units would (the sin / cos rows are
+    bounded by 1 at any scale)."""
     rng = np.random.default_rng(seed)
     w = {}
-    for name, n_out, n_in, wn in layer_table(n_kpt):
+    for name, n_out, n_in, wn in layer_table(n_kpt, sp_level):
         if wn:
             v = (rng.standard_normal((n_out, n_in)) * np.sqrt(2.0 / n_in)).astype(F32)
+            if dz_scale != 1.0 and name == "mlp_geo.layers1.layers.0.linear":
+                v[:, :n_kpt] = (v[:, :n_kpt] / np.float32(dz_scale)).astype(F32)
             w[name + ".weight_v"] = v
             w[name + ".weight_g"] = np.linalg.norm(v.astype(np.float64), axis=1, keepdims=True).astype(F32)
         else:
@@ -199,6 +206,14 @@ def make_weights(n_kpt: int = 18, seed: int = 26, density_gain: float = 30.0) ->
     return w
 
 
-def sp_args(n_kpt: int = 18) -> dict:
-    """``configs/zju.json:38-44`` with n_kpt overridden."""
-    return {"sp_level": 3, "sp_type": "rel_z_decay", "scale": 1.0, "sigma": 0.1, "n_kpt": n_kpt}
+def sp_args(n_kpt: int = 18, **overrides) -> dict:
+    """``configs/zju.json:38-44`` with n_kpt and any of ``sp_level`` / ``scale`` / ``sigma`` overridden; ``sigma=None`` leaves the
+    key out, so that the reference's default (150, ``src/spatial.py:112``) applies."""
+    sp = {"sp_level": 3, "sp_type": "rel_z_decay", "scale": 1.0, "sigma": 0.1, "n_kpt": n_kpt}
+    unknown = set(overrides) - {"sp_level", "scale", "sigma"}
+    if unknown:
+        raise ValueError(f"unknown sp_args overrides {sorted(unknown)}")
+    sp.update(overrides)
+    if sp["sigma"] is None:
+        del sp["sigma"]
+    return sp

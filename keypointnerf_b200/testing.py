@@ -6,12 +6,18 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from . import synthetic as syn
 from .config import default_cfg
 from .model import KeypointNeRF
 
 
-def build_model(weights: dict, n_kpt: int, device="cuda:0") -> KeypointNeRF:
-    net = KeypointNeRF(default_cfg(n_kpt))
+def build_model(weights: dict, n_kpt: int, device="cuda:0", sp_args: dict | None = None) -> KeypointNeRF:
+    """``sp_args``: overrides of the config's ``sp_level`` / ``scale`` / ``sigma`` (``synthetic.sp_args``; sigma None leaves the
+    key out, so the model takes the reference's default of 150)."""
+    cfg = default_cfg(n_kpt)
+    if sp_args:
+        cfg["models"]["KeypointNeRF"]["sp_args"] = syn.sp_args(n_kpt, **sp_args)
+    net = KeypointNeRF(cfg)
     sd = {k: torch.from_numpy(np.asarray(v)) for k, v in weights.items()}
     res = net.load_state_dict(sd, strict=False)
     assert not res.unexpected_keys, res.unexpected_keys

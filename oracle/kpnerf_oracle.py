@@ -225,13 +225,13 @@ def encode_rel_z_decay(scene: dict, pts: T, sp_level: int = 3, scale: float = 1.
     d2 = ((c[:, :, None, :] - ck[:, None, :, :]) ** 2).sum(-1)
     wk = torch.exp(-d2 / (2.0 * sigma ** 2))
     freqs = [np.float32(np.pi * (2 ** l)) if _DTYPE == torch.float32 else np.pi * (2 ** l) for l in range(sp_level)]
-    y = torch.stack([dz * float(f) for f in freqs], 2)  # (V,N,L,K)
     # reference layout: cat(sin(y), cos(y)) along the keypoint axis then flattened:
-    # [dz(K) | l0: sin(K) cos(K) | l1: sin cos | ...]  (src/spatial.py:35-39)
+    # [dz(K) | l0: sin(K) cos(K) | l1: sin cos | ...]  (src/spatial.py:35-39); sp_level 0 is the dz row alone (31-32)
     rows = [dz]
-    for l in range(sp_level):
-        rows.append(torch.sin(y[:, :, l]))
-        rows.append(torch.cos(y[:, :, l]))
+    for f in freqs:
+        y = dz * float(f)  # (V,N,K)
+        rows.append(torch.sin(y))
+        rows.append(torch.cos(y))
     enc = torch.stack(rows, 2) * wk[:, :, None, :]  # (V,N,1+2L,K)
     return enc.reshape(enc.shape[0], enc.shape[1], -1)
 

@@ -56,9 +56,12 @@ def import_reference():
     return M
 
 
-def build_net(M, n_kpt, weights):
+def build_net(M, n_kpt, weights, sp_args=None):
+    """The reference model with the given weights; ``sp_args`` (the whole dict, ``synthetic.sp_args``) replaces the config's."""
     cfg = json.load(open("/root/reference/configs/zju.json"))
     cfg["models"]["KeypointNeRF"]["sp_args"]["n_kpt"] = n_kpt
+    if sp_args is not None:
+        cfg["models"]["KeypointNeRF"]["sp_args"] = dict(sp_args)
     net = M.KeypointNeRF(cfg).eval()
     sd = {k: torch.from_numpy(np.asarray(v)) for k, v in weights.items()}
     res = net.load_state_dict(sd, strict=False)

@@ -32,6 +32,7 @@ TOL = {
     1: dict(rgb=1e-4, alpha=1e-4, contrib=1e-4, depth=2e-3, sdf=2e-3, q99_fine=1e-3, psnr=80.0),
 }
 TOL[4] = TOL[0]
+TOL[2] = TOL[0]   # engine 2: the tensor-core kernels without the density tail's W_lo term
 ALL = np.ones((), dtype=bool)   # every ray
 
 

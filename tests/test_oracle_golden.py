@@ -45,12 +45,13 @@ def test_fp64_oracle_meets_the_same_tolerances(case):
         check_tile_fine(case)
 
 
-def check_query_stages(case, f8_atol=1e-5):
+def check_query_stages(case, f8_atol=1e-5, sp=None):
+    """``sp``: the fixture's sp_args (sp_level / scale / sigma), the oracle's defaults when None; likewise below."""
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
     pts = torch.from_numpy(g["query_pts"])
     view = torch.from_numpy(g["query_view"])
-    out, valid, parts = O.query(scene, fw, pts, view, return_parts=True)
+    out, valid, parts = O.query(scene, fw, pts, view, sp, return_parts=True)
     sel = g["sel"]
     assert np.array_equal(valid.numpy(), g["query_valid"])
     np.testing.assert_allclose(parts["pw"][..., 0].numpy(), g["pw"], atol=2e-6)
@@ -60,7 +61,7 @@ def check_query_stages(case, f8_atol=1e-5):
     np.testing.assert_allclose(parts["x_view"].numpy()[:, sel], g["x_view"], atol=1e-4)
     np.testing.assert_allclose(parts["x_pool"].numpy()[sel], g["x_pool"], atol=1e-4)
     np.testing.assert_allclose(out[:, :2].numpy(), g["geo_out"], atol=2e-3, rtol=1e-4)  # density row has gain 30
-    f = torch.cat([parts["rgb_src"], parts["tex"], parts["lat"][None].expand(3, -1, -1)], -1)
+    f = torch.cat([parts["rgb_src"], parts["tex"], parts["lat"][None].expand(parts["rgb_src"].shape[0], -1, -1)], -1)
     np.testing.assert_allclose(f.permute(1, 0, 2).numpy()[sel], g["ibr_feat"], atol=1e-4)
     np.testing.assert_allclose(parts["ray_diff"].permute(1, 0, 2).numpy()[sel], g["ibr_raydiff"], atol=2e-5)
     v = g["query_valid"]
@@ -68,10 +69,10 @@ def check_query_stages(case, f8_atol=1e-5):
     np.testing.assert_allclose(out.numpy()[v], g["query_out"][v], atol=2e-3, rtol=1e-4)
 
 
-def check_tile_coarse(case):
+def check_tile_coarse(case, sp=None):
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
-    r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True)
+    r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True, sp)
     np.testing.assert_allclose(r["z"].numpy(), g["z_coarse"], atol=2e-6)
     np.testing.assert_allclose(r["rgba"].numpy(), g["rgba_coarse"], atol=2e-3, rtol=1e-4)
     np.testing.assert_allclose(r["contrib"].numpy(), g["contrib_coarse"], atol=2e-5)
@@ -80,17 +81,17 @@ def check_tile_coarse(case):
     np.testing.assert_allclose(r["depth"].numpy(), g["depth"][0], atol=2e-4)
 
 
-def check_tile_fine(case):
+def check_tile_fine(case, sp=None):
     g, meta, scene, weights, target = case
     fw = O.fold_weights(weights)
-    r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True)
+    r = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True, sp)
     # free-running hierarchical pass: inverse-CDF is discontinuous (SURVEY.md section 7 hard part 3), so
     # compare the resampled depths loosely and the image by PSNR ...
     dz = np.abs(r["z_fine"].numpy() - g["z_fine"])
     assert np.quantile(dz, 0.99) < 1e-4
     assert psnr(r["tex_fg_fine"].numpy(), g["tex_fg_fine"][0]) > 60.0
     # ... and tightly with the reference's own z_fine injected.
-    r2 = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True,
+    r2 = O.render_tile(scene, fw, target, meta["level"], meta["x_off"], meta["y_off"], meta["S_c"], meta["S_f"], True, sp,
                        z_fine_override=g["z_fine"])
     np.testing.assert_allclose(r2["tex_fg_fine"].numpy(), g["tex_fg_fine"][0], atol=3e-5)
     np.testing.assert_allclose(r2["alpha_fine"].numpy(), g["alpha_fine"][0], atol=3e-5)

@@ -77,13 +77,22 @@ def target_wh(meta):
 
 def scene_from_meta(meta):
     """Seeded scene, weights and target of a fixture.  ``src_height`` / ``tgt_width`` / ``tgt_height`` describe non-square
-    sources and targets; older fixtures do not have them and are square (``src_size`` / ``tgt_size``)."""
-    scene = syn.make_scene(src_size=meta["src_size"], n_views=3, n_kpt=meta["n_kpt"], seed=meta["scene_seed"],
+    sources and targets; older fixtures do not have them and are square (``src_size`` / ``tgt_size``).  ``n_views``,
+    ``sp_level`` and ``dz_scale`` default to 3, 3 and 1 (fixtures that predate them)."""
+    scene = syn.make_scene(src_size=meta["src_size"], n_views=meta.get("n_views", 3), n_kpt=meta["n_kpt"], seed=meta["scene_seed"],
                            fg_hole=meta["fg_hole"], fg_mode=meta.get("fg_mode", "ones"), src_height=meta.get("src_height"))
-    weights = syn.make_weights(meta["n_kpt"], seed=meta["w_seed"])
+    weights = syn.make_weights(meta["n_kpt"], seed=meta["w_seed"], sp_level=meta.get("sp_level", 3),
+                               dz_scale=meta.get("dz_scale", 1.0))
     w, h = target_wh(meta)
     target = syn.make_target(size=meta["tgt_size"], azimuth=meta["azimuth"], zoom=meta.get("zoom", 1.0), width=w, height=h)
     return scene, weights, target
+
+
+def sp_from_meta(meta):
+    """The fixture's ``sp_args`` overrides for ``testing.build_model`` (sigma None: left out of the config, so 150) and the same
+    parameters as the oracle's ``sp`` dict (which needs the value itself)."""
+    sp = {"sp_level": meta.get("sp_level", 3), "scale": meta.get("scale", 1.0), "sigma": meta.get("sigma", 0.1)}
+    return sp, dict(sp, sigma=150.0 if sp["sigma"] is None else sp["sigma"])
 
 
 def checksum(scene, weights):
