@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define KPN_ABI_VERSION 2
+#define KPN_ABI_VERSION 3
 #define KPN_MAX_VIEWS 4
 #define KPN_MAX_KPT 32
 #define KPN_NUM_LAYERS 19
@@ -143,6 +143,15 @@ typedef struct {
   int mem;             /* kpn_mem of the pointers above */
 } kpn_out;
 
+/* A regular grid of points: point (i,j,k), 0<=i<nx, 0<=j<ny, 0<=k<nz, has id (k*ny + j)*nx + i (x fastest) and position
+ * p[a] = origin[a] + spacing[a]*idx_a, computed in fp32 as one multiply then one add (no fused multiply-add), so that a
+ * caller can rebuild the points bit for bit. */
+typedef struct {
+  float origin[3];
+  float spacing[3];
+  int nx, ny, nz;
+} kpn_grid;
+
 typedef struct {
   uint64_t samples_total;   /* samples generated by the last render/query */
   uint64_t samples_valid;   /* samples that passed the validity test and were shaded */
@@ -182,6 +191,34 @@ int kpn_render(kpn_ctx* ctx, const kpn_target* target, const kpn_opts* opts, con
  * multiplied by a zero mask downstream, src/model.py:982,996). */
 int kpn_query(kpn_ctx* ctx, const float* pts, const float* view, int n, float* out5, uint8_t* valid,
               int mem, const kpn_opts* opts, void* stream);
+
+/* The density field of KeypointNeRF.query on a grid, without the colour branch: out2 (n,2) = [sdf_raw, rad] and valid (n)
+ * in {0,1}, n = nx*ny*nz, indexed by grid id.  No per-point input.  A point's [sdf_raw, rad, valid] is bit-identical to
+ * columns 0-1 of kpn_query at the same point with the same engine (the view direction only enters the colour).  Rows with
+ * valid==0 carry [0,0].  Same engines and shapes as kpn_query; n <= 2^31-1, every extent >= 1, spacing finite and > 0
+ * (else KPN_ERR_ARG).  kpn_get_stats reports samples_total = n, samples_valid, and samples_coloured = 0.
+ * `mem` = kpn_mem of out2 and valid (valid may be NULL). */
+int kpn_query_grid(kpn_ctx* ctx, const kpn_grid* grid, float* out2, uint8_t* valid, int mem, const kpn_opts* opts, void* stream);
+
+/* Marching cubes, first half: classifies the cells of the fp32 volume `field` (DEVICE pointer, f[nz][ny][nx], x fastest)
+ * against `level` and scans the per-point vertex and per-cell face counts; writes [n_vertices, n_faces] to counts (host).
+ * A corner is inside when f > level (NaN: outside); each grid edge with one inside endpoint gets one vertex.  The workspace
+ * (about 9 bytes per point) is kept in the context for kpn_mesh_emit.  More than 2^31-1 points, vertices or faces:
+ * KPN_ERR_ARG.  Synchronises `stream` (the counts are needed to size the outputs). */
+int kpn_mesh_begin(kpn_ctx* ctx, const float* field, int nx, int ny, int nz, float level, long long counts[2], void* stream);
+
+/* Marching cubes, second half: the mesh of the field passed to the last kpn_mesh_begin (the same pointer, unchanged since;
+ * otherwise KPN_ERR_STATE), on the grid origin / spacing (host arrays, as kpn_grid):
+ *   vertices (n_vertices,3): one per crossing edge, ordered by (linear index of the edge's lower endpoint a, axis x<y<z), at
+ *     p_a + t*(p_b - p_a) with t = (level - f_a)/(f_b - f_a) (an edge with a non-finite t gets its midpoint);
+ *   normals (n_vertices,3) or NULL: -grad f / |grad f| interpolated by t between the endpoints' gradients (central
+ *     differences inside the grid, one-sided at its border); a zero gradient, or one that a NaN or infinite sample enters,
+ *     gives (0,0,0);
+ *   faces (n_faces,3) int32 vertex indices, by cell linear index then case-table order, counter-clockwise seen from the side
+ *     where f <= level.  Closed and edge-manifold when f <= level on the grid boundary.
+ * `mem` = kpn_mem of vertices, normals, faces (which may be NULL when their count is 0). */
+int kpn_mesh_emit(kpn_ctx* ctx, const float* field, const float origin[3], const float spacing[3], float* vertices, float* normals,
+                  int* faces, int mem, void* stream);
 
 /* Counters of the last call (+ the shading-kernel timings accumulated since the previous
  * kpn_get_stats when profiling is on).  Synchronises `stream` (debug/bench only). */

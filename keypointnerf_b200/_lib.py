@@ -19,8 +19,9 @@ KPN_NUM_LAYERS = 19
 KPN_NHWC_FEAT64, KPN_NHWC_FEAT8, KPN_NHWC_FEATTEX = 1, 2, 4
 
 EXPORTS = ["kpn_abi_version", "kpn_create", "kpn_destroy", "kpn_last_error", "kpn_set_weights", "kpn_set_scene",
-           "kpn_render", "kpn_query", "kpn_get_stats", "kpn_set_profiling", "kpn_selftest_umma", "kpn_selftest_umma2", "kpn_debug_timing", "kpn_debug_kmap", "kpn_check_health", "kpn_reserve", "kpn_debug_stage_times", "kpn_decode_views"]
-KPN_ABI_VERSION = 2
+           "kpn_render", "kpn_query", "kpn_get_stats", "kpn_set_profiling", "kpn_selftest_umma", "kpn_selftest_umma2", "kpn_debug_timing", "kpn_debug_kmap", "kpn_check_health", "kpn_reserve", "kpn_debug_stage_times", "kpn_decode_views",
+           "kpn_query_grid", "kpn_mesh_begin", "kpn_mesh_emit"]
+KPN_ABI_VERSION = 3
 
 c_float_p = C.POINTER(C.c_float)
 c_u8_p = C.POINTER(C.c_uint8)
@@ -63,6 +64,10 @@ class KpnOut(C.Structure):
     _fields_ = [("tex_fg", C.c_void_p), ("depth", C.c_void_p), ("alpha", C.c_void_p),
                 ("tex_fg_fine", C.c_void_p), ("depth_fine", C.c_void_p), ("alpha_fine", C.c_void_p),
                 ("sdf", C.c_void_p), ("z_fine", C.c_void_p), ("contrib", C.c_void_p), ("mem", C.c_int)]
+
+
+class KpnGrid(C.Structure):
+    _fields_ = [("origin", C.c_float * 3), ("spacing", C.c_float * 3), ("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int)]
 
 
 class KpnStats(C.Structure):
@@ -109,6 +114,14 @@ def load() -> C.CDLL:
     lib.kpn_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                               C.POINTER(KpnOpts), C.c_void_p]
     lib.kpn_query.restype = C.c_int
+    lib.kpn_query_grid.argtypes = [C.c_void_p, C.POINTER(KpnGrid), C.c_void_p, C.c_void_p, C.c_int, C.POINTER(KpnOpts), C.c_void_p]
+    lib.kpn_query_grid.restype = C.c_int
+    lib.kpn_mesh_begin.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_longlong),
+                                   C.c_void_p]
+    lib.kpn_mesh_begin.restype = C.c_int
+    lib.kpn_mesh_emit.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_int, C.c_void_p]
+    lib.kpn_mesh_emit.restype = C.c_int
     lib.kpn_get_stats.argtypes = [C.c_void_p, C.POINTER(KpnStats), C.c_void_p]
     lib.kpn_get_stats.restype = C.c_int
     lib.kpn_set_profiling.argtypes = [C.c_void_p, C.c_int]

@@ -74,6 +74,15 @@ struct kpn_ctx {
   // records (alpha+sdf, rgb, compositing weight), the fine depths, the colour kernel's latent scratch + work list
   DevBuf ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
   DevBuf ws_out, ws_in;
+  // marching cubes: per-point vertex offsets, per-cell case bytes and face offsets, scan scratch; the state kpn_mesh_begin
+  // leaves for kpn_mesh_emit
+  DevBuf mc_vofs, mc_cases, mc_tofs, mc_tmp;
+  unsigned long long* d_mc_totals = nullptr;
+  unsigned long long* h_mc_totals = nullptr;   // pinned
+  const float* mc_field = nullptr;   // the field of the last successful kpn_mesh_begin
+  int mc_dims[3] = {0, 0, 0};
+  float mc_level = 0.0f;
+  long long mc_counts[2] = {0, 0};
   unsigned long long launches = 0;
   bool profiling = false;
   unsigned int* h_wd = nullptr;   // pinned host copy of the tensor-core kernels' watchdog words (refreshed by every render/query)
@@ -115,7 +124,9 @@ extern "C" int kpn_create(int device, kpn_ctx** out) {
             cudaMalloc(&c->d_target, sizeof(DevTarget)) == cudaSuccess &&
             cudaMalloc(&c->d_wf32, sizeof(DevWeightsF32)) == cudaSuccess &&
             cudaMalloc(&c->d_counters, sizeof(int) * MAX_CHUNKS) == cudaSuccess &&
-            cudaMalloc(&c->d_counters2, sizeof(int) * MAX_CHUNKS) == cudaSuccess;
+            cudaMalloc(&c->d_counters2, sizeof(int) * MAX_CHUNKS) == cudaSuccess &&
+            cudaMalloc(&c->d_mc_totals, 2 * sizeof(unsigned long long)) == cudaSuccess &&
+            cudaHostAlloc(reinterpret_cast<void**>(&c->h_mc_totals), 2 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
   if (!ok) { kpn_destroy(c); return KPN_ERR_CUDA; }
   cudaMemset(c->d_counters, 0, sizeof(int) * MAX_CHUNKS);
   cudaMemset(c->d_counters2, 0, sizeof(int) * MAX_CHUNKS);
@@ -133,7 +144,8 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   if (!c) return;
   DeviceGuard g(c->device);
   cudaFree(c->d_raw_scene); cudaFree(c->d_scene); cudaFree(c->d_raw_target); cudaFree(c->d_target);
-  cudaFree(c->d_wf32); cudaFree(c->d_counters); cudaFree(c->d_counters2);
+  cudaFree(c->d_wf32); cudaFree(c->d_counters); cudaFree(c->d_counters2); cudaFree(c->d_mc_totals);
+  if (c->h_mc_totals) cudaFreeHost(c->h_mc_totals);
   c->wbuf.release();
   c->wblob.release();
   c->wlo.release();
@@ -141,7 +153,8 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   for (auto& b : c->atlas) b.release();
   c->atlas_fg.release();
   for (DevBuf* b : {&c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
-                    &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in})
+                    &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in, &c->mc_vofs, &c->mc_cases, &c->mc_tofs,
+                    &c->mc_tmp})
     b->release();
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   if (c->h_wd) cudaFreeHost(c->h_wd);
@@ -660,7 +673,7 @@ extern "C" int kpn_query(kpn_ctx* c, const float* pts, const float* view, int n,
     memset(&src, 0, sizeof(src));
     src.mode = 1; src.pts = dp + 3 * off; src.view = dv + 3 * off;
     KPN_CUDA(c, c->ws_list.reserve((size_t)m * sizeof(int)));
-    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + 5 * off, dvalid + off, st));
+    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + 5 * off, 5, dvalid + off, st));
     c->launches++;
     ShadeOut so;
     memset(&so, 0, sizeof(so));
@@ -675,6 +688,125 @@ extern "C" int kpn_query(kpn_ctx* c, const float* pts, const float* view, int n,
     if (valid) KPN_CUDA(c, cudaMemcpyAsync(valid, dvalid, (size_t)n, cudaMemcpyDeviceToHost, st));
   }
   return wd_snapshot(c, st);
+}
+
+extern "C" int kpn_query_grid(kpn_ctx* c, const kpn_grid* g, float* out2, uint8_t* valid, int mem, const kpn_opts* op, void* stream) {
+  if (!c || !g || !out2) return KPN_ERR_ARG;
+  DeviceGuard dg(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->nx < 1 || g->ny < 1 || g->nz < 1 || (long long)g->nx * g->ny * g->nz > 0x7fffffffll)
+    KPN_FAIL(c, KPN_ERR_ARG, "grid %d x %d x %d: every extent >= 1, at most 2^31 - 1 points", g->nx, g->ny, g->nz);
+  for (int a = 0; a < 3; ++a)
+    if (!std::isfinite(g->origin[a]) || !std::isfinite(g->spacing[a]) || !(g->spacing[a] > 0.0f))
+      KPN_FAIL(c, KPN_ERR_ARG, "grid origin / spacing must be finite, spacing > 0 (axis %d: %g, %g)", a, g->origin[a], g->spacing[a]);
+  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_query_grid");
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  int rc = begin_counters(c, st);
+  if (rc != KPN_OK) return rc;
+  const long long n = (long long)g->nx * g->ny * g->nz;
+  float* dout = out2; uint8_t* dvalid = valid;
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, c->ws_out.reserve((size_t)n * 2 * sizeof(float) + (size_t)n));
+    dout = c->ws_out.as<float>();
+    dvalid = reinterpret_cast<uint8_t*>(c->ws_out.as<char>() + (size_t)n * 2 * sizeof(float));
+  } else if (!dvalid) {
+    KPN_CUDA(c, c->ws_out.reserve((size_t)n));
+    dvalid = c->ws_out.as<uint8_t>();
+  }
+  const long long chunk = 4ll << 20;   // as kpn_query
+  const long long nchunks = (n + chunk - 1) / chunk;
+  for (long long ch = 0; ch < nchunks; ++ch) {
+    const long long off = ch * chunk;
+    const long long m = (n - off) < chunk ? (n - off) : chunk;
+    SampleSrc src;
+    memset(&src, 0, sizeof(src));
+    src.mode = 2;
+    for (int a = 0; a < 3; ++a) { src.g_org[a] = g->origin[a]; src.g_sp[a] = g->spacing[a]; }
+    src.g_nx = g->nx; src.g_ny = g->ny; src.g_id0 = off;
+    KPN_CUDA(c, c->ws_list.reserve((size_t)m * sizeof(int)));
+    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + 2 * off, 2, dvalid + off, st));
+    c->launches++;
+    ShadeOut so;
+    memset(&so, 0, sizeof(so));
+    so.out2 = dout + 2 * off;
+    rc = shade_batch(c, src, c->ws_list.as<int>(), c->d_counters + ch, c->d_counters2 + ch, m, 2, so, op ? op->engine : 0, st);
+    if (rc != KPN_OK) return rc;
+  }
+  c->counters_used = (int)nchunks;
+  c->last_total = (unsigned long long)n;
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, cudaMemcpyAsync(out2, dout, (size_t)n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (valid) KPN_CUDA(c, cudaMemcpyAsync(valid, dvalid, (size_t)n, cudaMemcpyDeviceToHost, st));
+  }
+  return wd_snapshot(c, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// marching cubes (kpn_mesh.cu)
+// ---------------------------------------------------------------------------------------------
+extern "C" int kpn_mesh_begin(kpn_ctx* c, const float* field, int nx, int ny, int nz, float level, long long counts[2], void* stream) {
+  if (!c || !field || !counts) return KPN_ERR_ARG;
+  DeviceGuard dg(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  c->mc_field = nullptr;
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  if (nx < 1 || ny < 1 || nz < 1 || (long long)nx * ny * nz > 0x7fffffffll)
+    KPN_FAIL(c, KPN_ERR_ARG, "field %d x %d x %d: every extent >= 1, at most 2^31 - 1 points", nx, ny, nz);
+  const int n = nx * ny * nz;
+  const long long ncell = (long long)(nx - 1) * (ny - 1) * (nz - 1);
+  KPN_CUDA(c, c->mc_vofs.reserve((size_t)n * sizeof(unsigned int)));
+  KPN_CUDA(c, c->mc_cases.reserve(ncell > 0 ? (size_t)ncell : 1));
+  KPN_CUDA(c, c->mc_tofs.reserve((ncell > 0 ? (size_t)ncell : 1) * sizeof(unsigned int)));
+  const size_t scan_bytes = mc_scan_temp_bytes(n);
+  KPN_CUDA(c, c->mc_tmp.reserve(scan_bytes));
+  KPN_CUDA(c, launch_mc_classify(field, nx, ny, nz, level, c->mc_vofs.as<unsigned int>(), c->mc_cases.as<uint8_t>(),
+                                 c->mc_tofs.as<unsigned int>(), c->d_mc_totals, c->mc_tmp.p, scan_bytes, st));
+  c->launches += ncell > 0 ? 5 : 3;   // classify + CUB's two kernels per scan
+  KPN_CUDA(c, cudaMemcpyAsync(c->h_mc_totals, c->d_mc_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  KPN_CUDA(c, cudaStreamSynchronize(st));
+  const unsigned long long nv = c->h_mc_totals[0], nf = c->h_mc_totals[1];
+  if (nv > 0x7fffffffull || nf > 0x7fffffffull)
+    KPN_FAIL(c, KPN_ERR_ARG, "mesh of %llu vertices, %llu faces: at most 2^31 - 1 of each", nv, nf);
+  counts[0] = (long long)nv; counts[1] = (long long)nf;
+  c->mc_counts[0] = counts[0]; c->mc_counts[1] = counts[1];
+  c->mc_field = field;
+  c->mc_dims[0] = nx; c->mc_dims[1] = ny; c->mc_dims[2] = nz;
+  c->mc_level = level;
+  return KPN_OK;
+}
+
+extern "C" int kpn_mesh_emit(kpn_ctx* c, const float* field, const float origin[3], const float spacing[3], float* vertices,
+                             float* normals, int* faces, int mem, void* stream) {
+  if (!c || !field || !origin || !spacing) return KPN_ERR_ARG;
+  DeviceGuard dg(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  for (int a = 0; a < 3; ++a)
+    if (!std::isfinite(origin[a]) || !std::isfinite(spacing[a]) || !(spacing[a] > 0.0f))
+      KPN_FAIL(c, KPN_ERR_ARG, "origin / spacing must be finite, spacing > 0 (axis %d: %g, %g)", a, origin[a], spacing[a]);
+  if (c->mc_field == nullptr || c->mc_field != field)
+    KPN_FAIL(c, KPN_ERR_STATE, "kpn_mesh_begin on the same field must precede kpn_mesh_emit");
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  const long long nv = c->mc_counts[0], nf = c->mc_counts[1];
+  if ((nv > 0 && !vertices) || (nf > 0 && !faces)) KPN_FAIL(c, KPN_ERR_ARG, "null vertices / faces for a non-empty mesh");
+  float* dv = vertices; float* dn = normals; int* df = faces;
+  const size_t vb = (size_t)nv * 3 * sizeof(float), fb = (size_t)nf * 3 * sizeof(int);
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, c->ws_out.reserve(2 * vb + fb + 16));
+    dv = c->ws_out.as<float>();
+    dn = normals ? reinterpret_cast<float*>(c->ws_out.as<char>() + vb) : nullptr;
+    df = reinterpret_cast<int*>(c->ws_out.as<char>() + 2 * vb);
+  }
+  KPN_CUDA(c, launch_mc_emit(field, c->mc_dims[0], c->mc_dims[1], c->mc_dims[2], c->mc_level, origin, spacing, c->mc_vofs.as<unsigned int>(),
+                             c->mc_cases.as<uint8_t>(), c->mc_tofs.as<unsigned int>(), dv, dn, df, nf, st));
+  c->launches += nf > 0 ? 2 : 1;
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, cudaMemcpyAsync(vertices, dv, vb, cudaMemcpyDeviceToHost, st));
+    if (normals) KPN_CUDA(c, cudaMemcpyAsync(normals, dn, vb, cudaMemcpyDeviceToHost, st));
+    KPN_CUDA(c, cudaMemcpyAsync(faces, df, fb, cudaMemcpyDeviceToHost, st));
+  }
+  return KPN_OK;
 }
 
 extern "C" int kpn_get_stats(kpn_ctx* c, kpn_stats* stats, void* stream) {

@@ -28,8 +28,18 @@ __device__ __forceinline__ float sample_depth(const SampleSrc& src, long long id
 }
 
 // ---- sample fetch -----------------------------------------------------------------------------
+// GRID: the kernel may see grid sources (mode 2).  The render kernels are compiled without that branch, so that their code is
+// what it is without the grid source.
+template <bool GRID = false>
 __device__ __forceinline__ void fetch_sample(const SampleSrc& src, long long id, float p[3], float d[3]) {
-  if (src.mode == 0) {
+  if (GRID && src.mode == 2) {
+    const long long g = src.g_id0 + id;
+    const long long r = g / src.g_nx;
+    const int idx[3] = {(int)(g - r * src.g_nx), (int)(r % src.g_ny), (int)(r / src.g_ny)};
+#pragma unroll
+    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(src.g_org[a], __fmul_rn(src.g_sp[a], (float)idx[a]));
+    d[0] = 0.0f; d[1] = 0.0f; d[2] = 0.0f;
+  } else if (src.mode == 0) {
     long long r = id / src.S;
     float z = sample_depth(src, id, r);
     d[0] = src.ray_d[3 * r + 0]; d[1] = src.ray_d[3 * r + 1]; d[2] = src.ray_d[3 * r + 2];

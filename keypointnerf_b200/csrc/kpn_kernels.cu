@@ -367,8 +367,9 @@ front_kernel(const DevScene* __restrict__ scp, const DevTarget* __restrict__ tgp
 // ------------------------------------------------------------------------------------------------
 // validity + compaction of explicit points (KeypointNeRF.query)
 // ------------------------------------------------------------------------------------------------
+// out: out_w floats per point (5: query, 2: geometry-only query), zeroed on invalid rows
 __global__ void compact_kernel(const DevScene* __restrict__ sc, SampleSrc src, long long n, int* __restrict__ list,
-                               int* __restrict__ counter, float* __restrict__ out5, uint8_t* __restrict__ valid_out) {
+                               int* __restrict__ counter, float* __restrict__ out, int out_w, uint8_t* __restrict__ valid_out) {
   const DevScene& S = *sc;
   __shared__ int s_cnt[8];
   __shared__ int s_base;
@@ -378,11 +379,11 @@ __global__ void compact_kernel(const DevScene* __restrict__ sc, SampleSrc src, l
     if (i < n) {
       float p[3], d[3];
       Proj q[MAXV];
-      fetch_sample(src, i, p, d);
+      fetch_sample<true>(src, i, p, d);
       ok = sample_valid(S, p, q);
       if (!ok) {   // rows with valid == 0 carry zeros (the reference multiplies them by a zero mask downstream)
-        float* o = out5 + 5 * i;
-        o[0] = 0.f; o[1] = 0.f; o[2] = 0.f; o[3] = 0.f; o[4] = 0.f;
+        float* o = out + out_w * i;
+        for (int c = 0; c < out_w; ++c) o[c] = 0.f;
       }
       if (valid_out) valid_out[i] = ok ? 1 : 0;
     }
@@ -549,7 +550,7 @@ shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restr
       int id = list[base + min(t, nrows - 1)];
       s.Id[t] = id;
       float p[3], d[3];
-      fetch_sample(src, id, p, d);
+      fetch_sample<true>(src, id, p, d);
       float* o = s.P + t * 8;
       o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = d[0]; o[4] = d[1]; o[5] = d[2];
     }
@@ -616,12 +617,18 @@ shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restr
       }
     }
     __syncthreads();
-    dense_tile<ACT_NONE, 1>(W, L_CMP, s.A, LDA, s.Lat, 24);   // ibr_compress_gfeat (src/model.py:819)
+    if (query_mode != 2) dense_tile<ACT_NONE, 1>(W, L_CMP, s.A, LDA, s.Lat, 24);   // ibr_compress_gfeat (src/model.py:819)
     dense_tile<ACT_SP, 2>(W, L_DEN0, s.A, LDA, s.B, LDB);
     __syncthreads();
     dense_tile<ACT_SP, 2>(W, L_DEN1, s.B, LDB, s.A, LDA);
     __syncthreads();
     dense_tile<ACT_NONE, 1>(W, L_DEN2, s.A, LDA, s.Geo, 2);
+    if (query_mode == 2) {   // geometry only: [sdf_raw, rad], no colour stages
+      __syncthreads();
+      if (t < nrows) reinterpret_cast<float2*>(so.out2)[s.Id[t]] = make_float2(s.Geo[t * 2], s.Geo[t * 2 + 1]);
+      __syncthreads();
+      continue;
+    }
     // ---- 5. colour branch inputs (reference src/model.py:806-832)
     for (int idx = t; idx < V * TS; idx += NT) {
       int v = idx / TS, r = idx % TS;
@@ -962,9 +969,9 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr
                                                                             counter, ray_start, ray_cnt, ert);
   return cudaGetLastError();
 }
-cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out5,
+cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out, int out_w,
                            uint8_t* valid_out, cudaStream_t st) {
-  compact_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(sc, src, n, list, counter, out5, valid_out);
+  compact_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(sc, src, n, list, counter, out, out_w, valid_out);
   return cudaGetLastError();
 }
 template <int NV, int TS>

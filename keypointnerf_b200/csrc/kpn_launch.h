@@ -12,7 +12,7 @@ cudaError_t launch_prep_target(const RawTarget* raw, DevTarget* tg, const DevSce
 cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr, int S, const float* zbuf, float* ray_d,
                          float* ray_nf, int* list, int list_base, int* counter, int* ray_start, int* ray_cnt, const ErtSegment& ert,
                          cudaStream_t st);
-cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out5,
+cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out, int out_w,
                            uint8_t* valid_out, cudaStream_t st);
 cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,
                               const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
@@ -24,7 +24,7 @@ cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb
 cudaError_t launch_resample(const int* list, const float* cw, const int* start0, const int* cnt0, const int* start1, const int* cnt1,
                             const float* ray_nf, int nr, int Sc, int Sf, float* zout, float* contrib_out, cudaStream_t st);
 // Tensor-core engine: geometry front (L0-L3 + pooling) and density tail kernels, then the colour kernel on the samples with
-// density > 0.  n_views: 3 or 4 (the scene's view count, tc_supported); wblob: full fp16 W_hi tiles of every stage; wlo: W_lo
+// density > 0 (query_mode 2: no colour kernel).  n_views: 3 or 4 (the scene's view count, tc_supported); wblob: full fp16 W_hi tiles of every stage; wlo: W_lo
 // tiles of stages 4, 5 (tc_weight_lo_bytes); lat_scratch: n_max x 48 bytes, pool_scratch: tc_pool_bytes(n_max), list2:
 // n_max x int2, count2: device int (zeroed by the caller).  *launches is incremented by the number of kernels enqueued.
 cudaError_t launch_shade_tc(const DevScene* sc, int n_views, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term,
@@ -52,6 +52,15 @@ bool tc_supported(int n_views, int n_kpt, int sp_level);
 // source-view decode (kpn_decode.cu): cams = V x {double ir[9], fx, fy, cx, cy, k1, k2, p1, p2, k3} on the device
 cudaError_t launch_decode_views(const uint8_t* images, const uint8_t* masks, const void* cams, int V, int H0, int W0, int factor,
                                 float* out_img, uint8_t* out_mask, cudaStream_t st);
+// marching cubes (kpn_mesh.cu) over f[nz][ny][nx], nx * ny * nz <= INT32_MAX.  classify: vcnt (per point) and tcnt (per cell)
+// become the exclusive scans vofs / tofs, cases[cell] the case byte, totals[2] (device) = [vertices, faces]; scan_tmp holds
+// mc_scan_temp_bytes(nx * ny * nz) bytes.  emit: vertices / normals (may be nullptr) / faces at those offsets.
+size_t mc_scan_temp_bytes(int n);
+cudaError_t launch_mc_classify(const float* f, int nx, int ny, int nz, float level, unsigned int* vcnt, uint8_t* cases, unsigned int* tcnt,
+                               unsigned long long* totals, void* scan_tmp, size_t scan_bytes, cudaStream_t st);
+cudaError_t launch_mc_emit(const float* f, int nx, int ny, int nz, float level, const float origin[3], const float spacing[3],
+                           const unsigned int* vofs, const uint8_t* cases, const unsigned int* tofs, float* verts, float* normals,
+                           int* faces, long long n_faces, cudaStream_t st);
 int max_coarse_samples();
 int simt_max_kpt();
 int simt_max_geo_input();   // widest geometry-layer-0 input ((1 + 2 sp_level) n_kpt + 64) the fp32 engine's tile rows hold

@@ -68,7 +68,9 @@ __device__ __forceinline__ void tail_mma(float* d, const uint8_t* ahi, const uin
   tc::named_sync(bar_id, 128);
 }
 
-// whi: the blob's W_hi tile of stage 4 (stage 5's follows it)
+// whi: the blob's W_hi tile of stage 4 (stage 5's follows it).  GEO_ONLY: the geometry-only query (query_mode 2), which writes
+// so.out2 and keeps no latent; a template parameter, so that the render / query instantiation is unchanged.
+template <bool GEO_ONLY>
 __global__ void __launch_bounds__(GWG * 128, 1)
 geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ whi, const uint8_t* __restrict__ wlo, int lo_mask,
                 const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
@@ -156,8 +158,8 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
       }
     }
     // ---- outputs (eval_func, src/model.py:978-997): alpha / sdf and, where a colour will be needed (density > 0: a sample with
-    //      alpha == 0 composites with weight exactly 0, skipping its colour is exact; every valid sample in query mode), the
-    //      compressed latent at the sample's own list index
+    //      alpha == 0 composites with weight exactly 0, skipping its colour is exact; every valid sample in query mode; none in
+    //      geometry-only mode), the compressed latent at the sample's own list index
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       float g0 = gs[k], rad = rs[k];
@@ -167,6 +169,10 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
       rad += wp2[129];
       const long long si = t0 + 16 * wq + (lane >> 2) + 8 * k;
       if (si < end) {
+        if (GEO_ONLY) {
+          if ((lane & 3) == 0) reinterpret_cast<float2*>(so.out2)[list[si]] = make_float2(g0, rad);
+          continue;
+        }
         if ((lane & 3) == 0) {
           if (query_mode) {
             float* o = so.out5 + 5ll * list[si];
@@ -206,12 +212,14 @@ cudaError_t launch_geo_tail(const TcConsts& C, const uint8_t* wtail, const uint8
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(geo_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
+    cudaError_t e = cudaFuncSetAttribute(geo_tail_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(geo_tail_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
-  geo_tail_kernel<<<tc_grid((len + 63) / 64, GWG, num_sms), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len,
-                                                                                       pool, query_mode, so, lat);
+  auto kernel = query_mode == 2 ? geo_tail_kernel<true> : geo_tail_kernel<false>;
+  kernel<<<tc_grid((len + 63) / 64, GWG, num_sms), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len, pool,
+                                                                              query_mode, so, lat);
   return cudaGetLastError();
 }
 

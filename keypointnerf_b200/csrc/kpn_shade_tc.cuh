@@ -315,8 +315,9 @@ __device__ __forceinline__ void encode_pair(const SceneS<NV>& S, int v, int j, i
   for (int r = 0; r < 7; ++r) a[r] = tc::pack_h2(e0[r], e1[r]);
 }
 
-// One instantiation per view count NV and keypoint pair count NP (nk = 2 NP - 1 or 2 NP keypoints).
-template <int NV, int NP>
+// One instantiation per view count NV and keypoint pair count NP (nk = 2 NP - 1 or 2 NP keypoints); GRID: for grid sources
+// (kpn_query_grid), the others take rays and explicit points.
+template <int NV, int NP, bool GRID>
 __global__ void __launch_bounds__(front_wgs(2 * NP, NV) * 128, 1)
 geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __restrict__ wblob, SampleSrc src,
                  const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
@@ -348,7 +349,7 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
     const long long si = base + (long long)tile * FSPT + (wq & 1) * SPW + min(g, SPW - 1);
     const int id = list[min(si, end - 1)];
     float p[3], dd[3];
-    fetch_sample(src, id, p, dd);
+    fetch_sample<GRID>(src, id, p, dd);
     const Proj q = project_s(scs, v, p);
     const float bw = boundary_weight_fast(q);
     const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
@@ -754,7 +755,8 @@ cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const 
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NV, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
+    cudaError_t e = cudaFuncSetAttribute(geo_front_kernel<NV, NP, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(geo_front_kernel<NV, NP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_front);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(shade_color_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COL_SMEM);
     if (e != cudaSuccess) return e;
@@ -767,13 +769,15 @@ cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const 
   const long long nslices = n_max > POOL_SLICE ? (n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
   for (long long s = 0; s < nslices; ++s) {
     const long long base = s * POOL_SLICE, len = n_max - base < POOL_SLICE ? n_max - base : POOL_SLICE;
-    geo_front_kernel<NV, NP><<<tc_grid((len + FSPT - 1) / FSPT, FWG, num_sms), FWG * 128, smem_front, st>>>(sc, nk, wblob, src, list,
-                                                                                                          counter, base, len, pool);
+    auto front = src.mode == 2 ? geo_front_kernel<NV, NP, true> : geo_front_kernel<NV, NP, false>;
+    front<<<tc_grid((len + FSPT - 1) / FSPT, FWG, num_sms), FWG * 128, smem_front, st>>>(sc, nk, wblob, src, list, counter, base, len,
+                                                                                         pool);
     e = launch_geo_tail(C, wtail, wlo, lo_mask, list, counter, base, len, pool, query_mode, so, lat, num_sms, st);
     if (e != cudaSuccess) return e;
     *launches += 2;
   }
   if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
+  if (query_mode == 2) return cudaSuccess;   // geometry only: no colour work list, no colour kernel
   const int grid = tc_grid((n_max + SPT - 1) / SPT, CWG, num_sms);
   if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
     shade_color_kernel<NV><<<grid, CWG * 128, COL_SMEM, st>>>(sc, C, wcol, src, nullptr, list, counter, lat, query_mode, so);

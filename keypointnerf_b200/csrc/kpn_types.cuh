@@ -69,24 +69,39 @@ struct DevWeightsF32 {
   float ani_al_abs;
 };
 
-// Where the samples of a shading launch come from.
+// Where the samples of a shading launch come from.  The grid fields of mode 2 share storage with the pointers, which that mode
+// does not read, so that the struct (a kernel parameter of every shading kernel) keeps the layout of modes 0 and 1.
 struct SampleSrc {
-  int mode;            // 0: rays (p = o + d*z(ray, i)),  1: explicit points
+  int mode;            // 0: rays (p = o + d*z(ray, i)),  1: explicit points,  2: grid points (no view direction)
   int S;               // samples per ray (mode 0)
-  const float* ray_d;  // (R,3) unit directions
-  const float* z;      // (R,S) depths; nullptr: the coarse pass' uniform depths, recomputed from ray_nf (never stored)
-  const float* ray_nf; // (R,2) near/far along the ray (used when z == nullptr)
-  const float* pts;    // (n,3)   (mode 1)
-  const float* view;   // (n,3)   (mode 1)
-  const float* o;      // (3) ray origin on device (mode 0)
+  union {
+    struct {
+      const float* ray_d;  // (R,3) unit directions
+      const float* z;      // (R,S) depths; nullptr: the coarse pass' uniform depths, recomputed from ray_nf (never stored)
+      const float* ray_nf; // (R,2) near/far along the ray (used when z == nullptr)
+      const float* pts;    // (n,3)   (mode 1)
+      const float* view;   // (n,3)   (mode 1)
+      const float* o;      // (3) ray origin on device (mode 0)
+    };
+    struct {
+      float g_org[3], g_sp[3];   // grid origin and spacing (mode 2): p[a] = g_org[a] + g_sp[a] * idx_a, no FMA contraction
+      int g_nx, g_ny;            // grid extent along x, y (mode 2); point id0 + id is (k g_ny + j) g_nx + i
+      long long g_id0;           // grid id of the launch's sample 0 (mode 2)
+    };
+  };
 };
+static_assert(sizeof(SampleSrc) == 8 + 6 * sizeof(void*), "the grid fields fit in the pointers' storage");
 
 // Where a shading launch puts its per-sample results.
-//   query mode (KeypointNeRF.query): out5[id] = [sdf_raw, rad, r, g, b], dense by sample id.
+//   query mode (KeypointNeRF.query, query_mode 1): out5[id] = [sdf_raw, rad, r, g, b], dense by sample id.
+//   geometry-only query (query_mode 2): out2[id] = [sdf_raw, rad], dense by sample id; no colour work.
 //   render mode: compact records indexed by the sample's position in the work list (list_base + index): ao[pos] = (alpha, sdf),
 //   rgb[pos] = blended colour (written only for samples with alpha > 0).  Nothing is stored for invalid samples.
 struct ShadeOut {
-  float* out5;     // query mode, else nullptr
+  union {
+    float* out5;   // query mode, else nullptr
+    float* out2;   // geometry-only query mode, else nullptr
+  };
   float2* ao;      // render mode
   float* rgb;      // render mode, 3 floats per list position
   int list_base;   // absolute list position of this launch's first entry

@@ -16,6 +16,7 @@ dropped).  Out of scope (SURVEY.md section 8f.3): the training ``forward``.
 from __future__ import annotations
 
 import copy
+import math
 
 import torch
 import torch.nn as nn
@@ -371,6 +372,43 @@ class KeypointNeRF(nn.Module):
         side.synchronize()
         net.marcher().check_health()
         return frames
+
+    # ---- surface extraction (the reference's users run query on a grid + skimage.measure.marching_cubes) -------------
+    @staticmethod
+    def mesh_grid(bounds, resolution=256):
+        """The grid ``extract_mesh`` samples: spacing ``h = max extent / (resolution - 1)`` on every axis,
+        ``n_a = ceil(extent_a / h - 1e-6) + 1`` points along axis a, origin ``bounds[0]``.  Returns (origin, spacing, dims) as
+        Python floats / ints, dims = (nx, ny, nz)."""
+        b = torch.as_tensor(bounds).detach().reshape(2, 3).double().cpu()
+        lo, ext = b[0], b[1] - b[0]
+        if resolution < 2 or not bool(torch.all(ext > 0)):
+            raise ValueError("extract_mesh needs resolution >= 2 and bounds[1] > bounds[0] on every axis")
+        h = float(ext.max()) / (resolution - 1)
+        dims = tuple(int(math.ceil(float(e) / h - 1e-6)) + 1 for e in ext)
+        return tuple(float(x) for x in lo), (h, h, h), dims
+
+    @staticmethod
+    def extract_mesh(net, img_in, cam_in, sp_data, bounds, level, resolution=256, colors=True, src_foreground_mask=None,
+                     feat_geo=None, feat_tex=None):
+        """The subject's surface as a triangle mesh: the density ``valid * relu(rad)`` (reference ``src/model.py:978-997``; it
+        depends only on the point, being pooled over the source views) on ``mesh_grid(bounds, resolution)`` with ``net.engine``,
+        zero-padded by one voxel so that the surface closes at the box, then marching cubes at ``level`` on the device.
+        ``colors``: the RGB of ``query`` at every vertex seen along ``-normal``.  Returns a dict of device tensors:
+        ``vertices`` (V,3), ``faces`` (F,3) int32 (counter-clockwise seen from outside), ``normals`` (V,3) and ``colors`` (V,3)."""
+        if feat_geo is None:
+            feat_geo = net.attach_geo_feat(img_in, return_val=True)
+        if feat_tex is None:
+            feat_tex = net.attach_tex_feat(img_in, return_val=True)
+        m = net._bind_scene(cam_in, feat_geo, feat_tex, sp_data, img_in, src_foreground_mask, bounds)
+        origin, spacing, dims = KeypointNeRF.mesh_grid(bounds, resolution)
+        out, valid = m.query_grid(origin, spacing, dims, engine=net.engine)
+        field = torch.nn.functional.pad(out[..., 1].clamp_min(0.0) * valid, (1, 1, 1, 1, 1, 1))
+        porigin = tuple(o - h for o, h in zip(origin, spacing))
+        verts, faces, normals = m.marching_cubes(field, porigin, spacing, level, normals=True)
+        res = {"vertices": verts, "faces": faces, "normals": normals}
+        if colors:   # an empty mesh (level above every density) has no vertices to query
+            res["colors"] = m.query(verts, -normals, engine=net.engine)[0][:, 2:5] if verts.shape[0] else verts.new_zeros(0, 3)
+        return res
 
     # ---- one pass (reference src/model.py:942-1108) ----------------------------------------------
     @staticmethod

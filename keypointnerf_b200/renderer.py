@@ -220,6 +220,57 @@ class RayMarcher:
             self.check_health()
         return out, valid.bool()
 
+    def query_grid(self, origin, spacing, dims, engine: int = 0):
+        """Geometry-only ``query`` on the grid points ``origin + spacing * (i, j, k)`` (``kpn_query_grid``), ``dims`` = (nx, ny, nz).
+        Returns ``(out (nz,ny,nx,2) = [sdf_raw, rad], valid (nz,ny,nx) bool)`` on this context's device; the values equal columns
+        0-1 of ``query`` at the same points bit for bit."""
+        nx, ny, nz = (int(d) for d in dims)
+        if min(nx, ny, nz) < 1 or nx * ny * nz > 2 ** 31 - 1:   # refused before the outputs are allocated
+            raise L.KpnError(f"query_grid: grid {nx} x {ny} x {nz}: every extent >= 1, at most 2^31 - 1 points")
+        g = L.KpnGrid()
+        g.origin[:] = [float(x) for x in origin]
+        g.spacing[:] = [float(x) for x in spacing]
+        g.nx, g.ny, g.nz = nx, ny, nz
+        dev = torch.device("cuda", self.device)
+        n = nx * ny * nz
+        out = torch.empty(n * 2, dtype=torch.float32, device=dev)
+        valid = torch.empty(n, dtype=torch.uint8, device=dev)
+        op = L.KpnOpts()
+        op.engine = int(engine)
+        L.check(self.lib, self.ctx,
+                self.lib.kpn_query_grid(self.ctx, C.byref(g), out.data_ptr(), valid.data_ptr(), L.KPN_MEM_DEVICE, C.byref(op),
+                                        self._stream()), "kpn_query_grid")
+        return out.view(nz, ny, nx, 2), valid.view(nz, ny, nx).bool()
+
+    def marching_cubes(self, field: torch.Tensor, origin, spacing, level: float, normals: bool = True):
+        """Marching cubes of ``field`` (nz,ny,nx) at ``level`` (inside: f > level) on the grid ``origin + spacing * (i, j, k)``
+        (``kpn_mesh_begin`` + ``kpn_mesh_emit``).  Returns ``(vertices (V,3) float32, faces (F,3) int32, normals (V,3) float32
+        or None)`` on the field's device (a host field is meshed on this context's device and the results are copied back);
+        faces are counter-clockwise seen from the side where f <= level.  Synchronises the current stream once (the counts size
+        the outputs)."""
+        f = _f32c(field)
+        if f.dim() != 3:
+            raise ValueError(f"field must be (nz, ny, nx), got {tuple(f.shape)}")
+        dev = torch.device("cuda", self.device)
+        if f.device != dev:
+            f = f.to(dev)
+        nz, ny, nx = f.shape
+        counts = (C.c_longlong * 2)()
+        L.check(self.lib, self.ctx,
+                self.lib.kpn_mesh_begin(self.ctx, f.data_ptr(), nx, ny, nz, float(level), counts, self._stream()), "kpn_mesh_begin")
+        nv, nf = int(counts[0]), int(counts[1])
+        verts = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        nrm = torch.empty(nv, 3, dtype=torch.float32, device=dev) if normals else None
+        faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+        o = (C.c_float * 3)(*[float(x) for x in origin])
+        h = (C.c_float * 3)(*[float(x) for x in spacing])
+        L.check(self.lib, self.ctx,
+                self.lib.kpn_mesh_emit(self.ctx, f.data_ptr(), o, h, verts.data_ptr(), nrm.data_ptr() if normals else None,
+                                       faces.data_ptr(), L.KPN_MEM_DEVICE, self._stream()), "kpn_mesh_emit")
+        self._keep_call = [f]
+        out_dev = field.device
+        return verts.to(out_dev), faces.to(out_dev), (nrm.to(out_dev) if normals else None)
+
     # ---- source-view decode (reference ZJUDataset.__getitem__, src/zju_dataset.py:266-287) ----------
     def decode_views(self, images: torch.Tensor, masks: torch.Tensor | None, K, D, ratio: float = 0.5):
         """Undistort + resize + mask every source view on the device (bit-identical to the reference's cv2 calls).
