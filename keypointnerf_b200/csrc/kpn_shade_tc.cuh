@@ -182,6 +182,22 @@ __device__ __forceinline__ void a_put(uint8_t* tile, int r, int c0, const uint32
 __device__ __forceinline__ void a_word(uint8_t* tile64, int r, int c, uint32_t w) {
   *reinterpret_cast<uint32_t*>(tile64 + tc::a_word_off<64>(r, c)) = w;
 }
+// store words [C0, C0 + N) of row r of a 64-row tile: whole 16-byte chunks as one store, the words of a chunk the run shares with
+// another writer one at a time
+template <int C0, int N>
+__device__ __forceinline__ void a_put_span(uint8_t* tile64, int r, const uint32_t* w) {
+#pragma unroll
+  for (int ch = C0 / 4; ch < (C0 + N + 3) / 4; ++ch) {
+    if (4 * ch >= C0 && 4 * ch + 4 <= C0 + N) {
+      const int i = 4 * ch - C0;
+      *reinterpret_cast<uint4*>(tile64 + tc::a_word_off<64>(r, 4 * ch)) = make_uint4(w[i], w[i + 1], w[i + 2], w[i + 3]);
+    } else {
+#pragma unroll
+      for (int c = 4 * ch; c < 4 * ch + 4; ++c)
+        if (c >= C0 && c < C0 + N) a_word(tile64, r, c, w[c - C0]);
+    }
+  }
+}
 // the activation tile written by this warpgroup's threads becomes visible to its MMAs
 __device__ __forceinline__ void wg_publish(int bar_id) {
   tc::fence_proxy_async_smem();
@@ -248,9 +264,10 @@ static_assert(64 * D3S * 4 <= 64 * 144 * 2, "the L3 rows fit in the activation t
 // up to three.  The row threads' gathers are latency bound, so a third warpgroup helps hide them; the register file caps the
 // CTA at three (168 registers per thread at 384 threads).  Three tiles fit up to K0P 208 (20 keypoints: 223 232 B dynamic +
 // the static scene block), two up to 28 keypoints (229 376 B), one above (29..32 keypoints: K0P 288 / 304).
-// Three warpgroups also need K0P >= 192 (15..20 keypoints): with narrower layer-0 inputs the split puts up to all 64 feat64
-// channels (64 LDG.128 taps) on one thread of a row, and built for 168 registers ptxas spills or serialises the wgmma chain of some
-// of those pair counts (NP 1, 2, 4 with 3 views; 4, 7 with 4 views), so 1..14 keypoints keep two.
+// Three warpgroups also need K0P >= 192 (15..20 keypoints): when the feat64 taps were loaded by the row's own threads, narrower
+// layer-0 inputs put up to all 64 channels (64 LDG.128) on one thread of a row, and built for 168 registers ptxas spilled or
+// serialised the wgmma chain of some of those pair counts, so 1..14 keypoints keep two.  gather_feat64 now spreads the taps
+// evenly over both warps of a row; three warpgroups for 1..14 keypoints have not been compiled and measured since.
 constexpr uint32_t SMEM_OPTIN = 227u * 1024u;
 // static shared memory of the front kernel (SceneS<NV> + mbarrier, ptxas): 2 000 B with 3 views, 2 624 B with 4
 constexpr uint32_t FRONT_STATIC_V3 = 2048u;
@@ -315,6 +332,74 @@ __device__ __forceinline__ void encode_pair(const SceneS<NV>& S, int v, int j, i
   for (int r = 0; r < 7; ++r) a[r] = tc::pack_h2(e0[r], e1[r]);
 }
 
+// feat64 channels of the layer-0 input (reference src/utils.py:74-89), loaded a whole 128-byte line per row at a time.  The row
+// warps wq and wq + 2 hold the same 32 rows (lane = row); warp h gathers all 64 channels of its lanes 16h .. 16h + 15, four rows
+// per step: lanes 8g .. 8g + 7 take row 16h + 4k + g of step k, and lane l8 = lane & 7 loads float4 groups l8 and l8 + 8 of that
+// row's four taps (each load instruction reads four whole lines, one per row; with a lane per row it read ~30 lines of 16 bytes
+// each).  The row's tap offsets and weights come from its lane by shuffles.  Each channel is blended with gather_f32's
+// expression and packed with the same pairs, and each word goes to the column tc_kmap gives it: channel c < FA to word
+// 7 PA + c/2 (thread 0's run), c >= FA to word C1 + NE + (c - FA)/2 (thread 1's run, after its NE encoding words).
+template <int NV, int NP>
+__device__ __forceinline__ void gather_feat64(const MapDesc& m, const Taps& t, uint8_t* A, int row0, int h, int lane) {
+  constexpr int NK = 2 * NP, PA = tc_l0_pa(NK), FA = tc_l0_fa(NK), C1 = 7 * PA + FA / 2, NE = 7 * (NP - PA);
+  static_assert(PA % 2 == 0 && FA % 4 == 0 && C1 % 2 == 0, "thread 0's feature words start on an even column");
+  const int o[4] = {t.o00, t.o01, t.o10, t.o11};   // texel offsets within the view's plane
+  const size_t plane = (size_t)m.H * m.W;
+  const float4* base = reinterpret_cast<const float4*>(m.ptr);
+  const int l8 = lane & 7;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int src = 16 * h + 4 * k + (lane >> 3);
+    const float4* vb = base + (size_t)(src % NV) * plane * 16;   // the row's view (lane = NV g + v); 16 float4 per texel
+    const float4* p[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) p[i] = vb + (size_t)__shfl_sync(FULL, o[i], src) * 16;
+    const float w00 = __shfl_sync(FULL, t.w00, src), w01 = __shfl_sync(FULL, t.w01, src);
+    const float w10 = __shfl_sync(FULL, t.w10, src), w11 = __shfl_sync(FULL, t.w11, src);
+    const int r = row0 + src;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int c4 = l8 + 8 * i;
+      const float4 a = __ldg(p[0] + c4), b = __ldg(p[1] + c4), c = __ldg(p[2] + c4), d = __ldg(p[3] + c4);
+      const uint32_t x0 = tc::pack_h2(a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11, a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11);
+      const uint32_t x1 = tc::pack_h2(a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11, a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11);
+      const int col = 4 * c4 < FA ? 7 * PA + 2 * c4 : C1 + NE + 2 * (c4 - FA / 4);
+      if (NE % 2 == 1 && (col & 1)) {
+        a_word(A, r, col, x0);
+        a_word(A, r, col + 1, x1);
+      } else {
+        *reinterpret_cast<uint2*>(A + tc::a_word_off<64>(r, col)) = make_uint2(x0, x1);
+      }
+    }
+  }
+}
+
+// feat8 channels [4h, 4h + 4) of the layer-2 input as two packed words (gather_f32's blend, same pairs as the 8-channel gather)
+template <int NV>
+__device__ __forceinline__ void gather_feat8(const SceneS<NV>& S, int v, const Proj& q, int h, uint32_t w[2]) {
+  const Taps t8 = make_taps(q.u, q.v, S.f8.W, S.f8.H);
+  float g8[4];
+  gather_f32<1>(S.f8, v, t8, h, g8);
+  w[0] = tc::pack_h2(g8[0], g8[1]);
+  w[1] = tc::pack_h2(g8[2], g8[3]);
+}
+
+// Latency options of a front instantiation's tile chain:
+//   FO_F8_EARLY     the feat8 words are gathered at the start of the tile, beside the feat64 gather, and held until the layer-2
+//                   input is built (otherwise they are gathered there, and the chain waits on a global load between L1 and L2);
+//   FO_NEXT_ID      the next tile's work-list entry is loaded at the start of the tile, so the tile after it starts on one global
+//                   load (the sample) instead of two dependent ones;
+//   FO_NEXT_SAMPLE  (with FO_NEXT_ID) the next tile's sample is also fetched, after L3, so a tile starts on no global load.
+// Each holds registers across the wgmma chain, and for some instantiations that makes ptxas serialise the chain's wgmma
+// instructions (warning C7511).  The table gives each instantiation the first of 7, 3, 6, 1, 2, 0 with which ptxas (CUDA 12.9,
+// -Xptxas -v) builds it without C7511 and without spills; every front instantiation compiles without C7511.  One digit per
+// pair count NP = 1 .. 16.
+constexpr int FO_F8_EARLY = 1, FO_NEXT_ID = 2, FO_NEXT_SAMPLE = 4;
+__host__ __device__ constexpr int front_opts(int nv, int np, bool grid) {
+  const char* t = nv <= 3 ? (grid ? "3777716677777737" : "7773777731776337") : (grid ? "1736777767773766" : "7777777737777737");
+  return t[np - 1] - '0';
+}
+
 // One instantiation per view count NV and keypoint pair count NP (nk = 2 NP - 1 or 2 NP keypoints); GRID: for grid sources
 // (kpn_query_grid), the others take rays and explicit points.
 template <int NV, int NP, bool GRID>
@@ -345,54 +430,69 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
   const int row = (wq & 1) * 32 + lane, h = wq >> 1;
   const int g = lane / NV, v = lane - NV * g;         // 3 views: lanes 30, 31 replay views 0, 1 of the warp's last sample (unused)
   const Group<NV> grp(lane);
-  for (int tile = blockIdx.x * FWG + wg; tile < ntiles; tile += gridDim.x * FWG) {
-    const long long si = base + (long long)tile * FSPT + (wq & 1) * SPW + min(g, SPW - 1);
-    const int id = list[min(si, end - 1)];
-    float p[3], dd[3];
-    fetch_sample<GRID>(src, id, p, dd);
+  const int tile0 = blockIdx.x * FWG + wg, tstride = gridDim.x * FWG;
+  const long long srow = (wq & 1) * SPW + min(g, SPW - 1);   // this lane's sample within a tile
+  constexpr int OPT = front_opts(NV, NP, GRID);
+  constexpr bool F8_EARLY = (OPT & FO_F8_EARLY) != 0, NEXT_ID = (OPT & FO_NEXT_ID) != 0;
+  constexpr bool NEXT_SAMPLE = NEXT_ID && (OPT & FO_NEXT_SAMPLE) != 0;
+  // the tile ahead's work-list entry (and sample) are fetched while the current tile runs; past the end the fetch is clamped to
+  // the last entry and not used
+  int idn = 0;
+  float pn[3] = {0.0f, 0.0f, 0.0f};
+  if constexpr (NEXT_ID) {
+    idn = list[min(base + (long long)tile0 * FSPT + srow, end - 1)];
+    if constexpr (NEXT_SAMPLE) {
+      float dd[3];
+      fetch_sample<GRID>(src, idn, pn, dd);
+    }
+  }
+  for (int tile = tile0; tile < ntiles; tile += tstride) {
+    const long long si = base + (long long)tile * FSPT + srow;
+    float p[3];
+    if constexpr (NEXT_SAMPLE) {
+      p[0] = pn[0]; p[1] = pn[1]; p[2] = pn[2];
+    } else {
+      float dd[3];
+      fetch_sample<GRID>(src, NEXT_ID ? idn : list[min(si, end - 1)], p, dd);
+    }
+    if constexpr (NEXT_ID) idn = list[min(si + (long long)tstride * FSPT, end - 1)];
     const Proj q = project_s(scs, v, p);
     const float bw = boundary_weight_fast(q);
     const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
-    // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap
+    uint32_t f8w[2];
+    if constexpr (F8_EARLY) gather_feat8(scs, v, q, h, f8w);
+    // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap:
+    //      this thread writes the encodings of its run (and thread 1 the bias column and K padding), gather_feat64 the feat64
+    //      words of both runs
     {
       float c[3];
       const float* E = scs.E[v];
       c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
       c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
       c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
-      const Taps t64 = make_taps(q.u, q.v, scs.f64.W, scs.f64.H);
+      gather_feat64<NV, NP>(scs.f64, make_taps(q.u, q.v, scs.f64.W, scs.f64.H), A, (wq & 1) * 32, h, lane);
       constexpr int C1 = 7 * PA + FA / 2;             // thread 0's run: words [0, C1); thread 1's: [C1, K0P / 2)
       static_assert(C1 % 4 == 0 && C1 > 0, "both runs start on a 16-byte chunk");
       if (h == 0) {
-        uint32_t a[C1];
+        if constexpr (PA > 0) {
+          uint32_t a[7 * PA];
 #pragma unroll
-        for (int gq = 0; gq < FA / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(scs.f64, v, t64, gq, f);
-          a[7 * PA + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[7 * PA + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
+          for (int j = 0; j < PA; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * j);
+          a_put_span<0, 7 * PA>(A, row, a);
         }
-#pragma unroll
-        for (int j = 0; j < PA; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * j);
-        a_put<64, C1>(A, row, 0, a);
       } else {
         constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
         constexpr int N1 = tc_k0p(NK) / 2 - C1;
         static_assert(NE + NF + 1 <= N1, "the bias column is in thread 1's run");
-        uint32_t a[N1];
-#pragma unroll
-        for (int gq = 0; gq < (64 - FA) / 4; ++gq) {
-          float f[4];
-          gather_f32<1>(scs.f64, v, t64, FA / 4 + gq, f);
-          a[NE + 2 * gq] = tc::pack_h2(f[0], f[1]);
-          a[NE + 2 * gq + 1] = tc::pack_h2(f[2], f[3]);
-        }
+        uint32_t a[NE > 0 ? NE : 1];
 #pragma unroll
         for (int j = PA; j < NP; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * (j - PA));
-        a[NE + NF] = H2_ONE;
+        if constexpr (NE > 0) a_put_span<C1, NE>(A, row, a);
+        uint32_t b[N1 - NE - NF];
+        b[0] = H2_ONE;
 #pragma unroll
-        for (int i = NE + NF + 1; i < N1; ++i) a[i] = 0u;
-        a_put<64, N1>(A, row, C1, a);
+        for (int i = 1; i < N1 - NE - NF; ++i) b[i] = 0u;
+        a_put_span<C1 + NE + NF, N1 - NE - NF>(A, row, b);
       }
     }
     // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720)
@@ -405,18 +505,19 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
     }
     front_mma<128, 9>(d, A, W + plan.st[1].off, bar_id);
     front_epi_sp(d, A, wq, lane, false);
-    if (h == 1) {   // layer-2 input: feat8 | bias chunk
-      uint32_t b[8] = {0u, 0u, 0u, 0u, H2_ONE, 0u, 0u, 0u};
-      const Taps t8 = make_taps(q.u, q.v, scs.f8.W, scs.f8.H);
-      float g8[8];
-      gather_f32<2>(scs.f8, v, t8, 0, g8);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) b[i] = tc::pack_h2(g8[2 * i], g8[2 * i + 1]);
-      a_put<64, 8>(A, row, 64, b);
+    {   // layer-2 input: feat8 (words 64 + 2h, 65 + 2h from this thread) | bias chunk (thread 1)
+      if constexpr (!F8_EARLY) gather_feat8(scs, v, q, h, f8w);
+      const uint32_t b[6] = {f8w[0], f8w[1], H2_ONE, 0u, 0u, 0u};
+      if (h == 0) a_put_span<64, 2>(A, row, b);
+      else a_put_span<66, 6>(A, row, b);
     }
     front_mma<128, 9>(d, A, W + plan.st[2].off, bar_id);
     front_epi_sp(d, A, wq, lane, true);
     front_mma<64, 8>(d, A, W + plan.st[3].off, bar_id);
+    if constexpr (NEXT_SAMPLE) {   // the next tile's sample (its work-list entry was loaded above)
+      float dd[3];
+      fetch_sample<GRID>(src, idn, pn, dd);
+    }
     // ---- L3 rows to shared memory (over the dead activation tile), then the view pooling: weighted mean || variance over
     //      the NV lanes of the group (src/utils.py:722-748); this thread owns 32 of the 64 feature columns
 #pragma unroll
