@@ -26,14 +26,16 @@ from keypointnerf_b200 import synthetic as syn
 from keypointnerf_b200.testing import build_model, scene_tensors
 from oracle import kpnerf_oracle as O  # checker only
 from tests import chunk_worker
+from tests.util import COLOUR_WGS, TAIL_WGS, front_wgs, tile_samples
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-# samples per tile of the geometry front kernel, the density tail and the colour kernel; 2 warpgroups (CTAs) per SM
-TILE_ROWS = (20, 64, 40)
-CTAS_PER_SM = 2
+# samples per tile and warpgroups per CTA (one CTA per SM) of the geometry front kernel at 18 keypoints, the density tail and
+# the colour kernel
+TILE_ROWS = tile_samples(3)
+WGS = (front_wgs(18), TAIL_WGS, COLOUR_WGS)
 
 # Per-sample gates against the fp64 oracle, per engine and output.  Largest errors measured on an H100 (all families):
 #   engine 0 (wgmma, two-term density tail): sdf 9.13e-4, rad 2.62e-2, rgb 5.60e-5.  The rad gate stays at the 5e-2 the other
@@ -130,8 +132,8 @@ def pool(bench):
 def batch_sizes():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ns = {1, 2, 19, 20, 21, 39, 40, 41, 63, 64, 65, 127, 128, 129}
-    for rows in TILE_ROWS:
-        wave = sms * CTAS_PER_SM * rows   # one full persistent wave of the kernel
+    for rows, wgs in zip(TILE_ROWS, WGS):
+        wave = sms * wgs * rows   # one full persistent wave of the kernel
         ns |= {wave - 1, wave, wave + 1, 2 * wave + 1}
     return sorted(ns)
 

@@ -19,14 +19,15 @@ from oracle import kpnerf_oracle as O  # checker only
 from tests import test_gpu_parity as P
 from tests.test_gpu_coverage import GATE
 from tests.test_gpu_kpt import _valid_count
-from tests.util import checksum, load_golden, psnr, target_wh
+from tests.util import COLOUR_WGS, TAIL_WGS, checksum, front_wgs, load_golden, psnr, target_wh, tile_samples
 
 pytestmark = pytest.mark.gpu
 
 ENGINES = [0, 1]
-# samples per tile with 4 views: geometry front kernel, density tail, colour kernel; 2 warpgroups (CTAs) per SM
-TILE_ROWS = (16, 64, 32)
-CTAS_PER_SM = 2
+# samples per tile with 4 views and warpgroups per CTA (one CTA per SM) of the geometry front kernel at 18 keypoints, the density
+# tail and the colour kernel
+TILE_ROWS = tile_samples(4)
+WGS = (front_wgs(18), TAIL_WGS, COLOUR_WGS)
 
 
 def scene_from_meta_views(meta):
@@ -158,8 +159,8 @@ def bench4():
 def _batch_sizes():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ns = {1, 2, 15, 16, 17, 31, 32, 33, 63, 64, 65}
-    for rows in TILE_ROWS:
-        wave = sms * CTAS_PER_SM * rows   # one full persistent wave of the kernel
+    for rows, wgs in zip(TILE_ROWS, WGS):
+        wave = sms * wgs * rows   # one full persistent wave of the kernel
         ns |= {wave - 1, wave, wave + 1, 2 * wave + 1}
     return sorted(ns)
 

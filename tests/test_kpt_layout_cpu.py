@@ -70,14 +70,57 @@ def test_weight_packing_is_a_bijection_for_every_count(lib, n_kpt):
     assert lib.kpn_debug_kmap(6, n_kpt, 64, buf, None, None) != 0
 
 
+def front_writers(pa, fa, c1, kpad, n_kpt):
+    """The words of a layer-0 row that each writer of geo_front_kernel stores, restated from the kernel: row thread h = 0 its
+    pairs' encodings (a_put_span<0, 7 PA>), row thread h = 1 its pairs' encodings (a_put_span<C1, NE>) and the bias column with
+    the K padding after the feat64 channels FA..63 (a_put_span<C1 + NE + NF, K0P / 2 - C1 - NE - NF>), and gather_feat64 the two
+    words of each float4 group c4 of feat64 channels at column 7 PA + 2 c4 (c4 < FA / 4) or C1 + NE + 2 (c4 - FA / 4)."""
+    ne, nf = 7 * ((n_kpt + 1) // 2 - pa), (64 - fa) // 2
+    w = {"h0 encodings": range(0, 7 * pa), "h1 encodings": range(c1, c1 + ne),
+         "h1 bias / padding": range(c1 + ne + nf, kpad // 2)}
+    for c4 in range(16):
+        col = 7 * pa + 2 * c4 if 4 * c4 < fa else c1 + ne + 2 * (c4 - fa // 4)
+        w[f"feat64 group {c4}"] = range(col, col + 2)
+    return w
+
+
+def assert_partition(writers, n_words):
+    """Every word of [0, n_words) is stored by exactly one writer, and no writer stores outside it."""
+    who = [[] for _ in range(n_words)]
+    for name, words in writers.items():
+        for c in words:
+            assert 0 <= c < n_words, f"{name} stores word {c}, outside [0, {n_words})"
+            who[c].append(name)
+    wrong = {c: names for c, names in enumerate(who) if len(names) != 1}
+    assert not wrong, f"words not stored exactly once: {wrong}"
+
+
 @pytest.mark.parametrize("n_kpt", COUNTS)
 def test_layer0_runs_are_chunk_aligned(lib, n_kpt):
     """The two row threads of the front kernel write one contiguous run of 32-bit words each, with 16-byte stores: both runs
-    start on a 4-word chunk and both have a whole number of chunks; the first thread gathers whole float4 groups of feat64."""
+    start on a 4-word chunk and both have a whole number of chunks; the first thread gathers whole float4 groups of feat64.
+    The L3 rows of a tile are staged over its activation tile, so every word of the next tile's layer-0 input must be stored
+    again: the front kernel's writers cover the row exactly once, each feat64 word at the column the weights expect, and the
+    same holds for words 64..71 of the layer-1 and layer-2 inputs (after the epilogue's words 0..63)."""
     km, kbias, kpad = kmap(lib, 0, n_kpt, n_inputs(0, n_kpt))
     pa, fa, c1 = layer0_runs(km, kbias, kpad, n_kpt)
     assert pa % 2 == 0 and fa % 4 == 0 and 0 < c1 < kpad // 2
     assert c1 % 4 == 0 and (kpad // 2 - c1) % 4 == 0
+    writers = front_writers(pa, fa, c1, kpad, n_kpt)
+    assert_partition(writers, kpad // 2)
+    feat = km[7 * n_kpt:]
+    for c in range(64):   # float4 group c // 4 packs channels (4g, 4g + 1) in its first word, (4g + 2, 4g + 3) in its second
+        assert feat[c] == 2 * writers[f"feat64 group {c // 4}"][(c % 4) // 2] + c % 2, c
+    assert kbias == 2 * writers["h1 bias / padding"][0]   # the H2_ONE word: 1.0 in the low half
+    # layer 1: the epilogue's words 0..63, the bias chunk of thread h = 0 (a_put<64, 8>)
+    k1, kb1, kp1 = kmap(lib, 1, n_kpt, n_inputs(1, n_kpt))
+    assert_partition({"epilogue": range(0, 64), "h0 bias chunk": range(64, 72)}, kp1 // 2)
+    assert k1.tolist() == list(range(128)) and kb1 == 128
+    # layer 2: the epilogue's words 0..63, feat8 channels 0..3 from thread h = 0 (a_put_span<64, 2>), channels 4..7, the bias
+    # column and the padding from thread h = 1 (a_put_span<66, 6>)
+    k2, kb2, kp2 = kmap(lib, 2, n_kpt, n_inputs(2, n_kpt))
+    assert_partition({"epilogue": range(0, 64), "h0 feat8": range(64, 66), "h1 feat8 / bias / padding": range(66, 72)}, kp2 // 2)
+    assert k2.tolist() == list(range(136)) and kb2 == 2 * 68
     # an odd count's last pair has one unused slot: nothing maps to the high half of its words
     if n_kpt % 2:
         j = n_kpt // 2

@@ -104,6 +104,23 @@ def checksum(scene, weights):
     return h.hexdigest()
 
 
+# Warpgroups per CTA of the tensor-core engine's kernels, which launch at most one CTA per SM (kpn_shade_tc.cuh): the geometry
+# front kernel's depend on the keypoint count (front_wgs there, the same for 3 and 4 views), the density tail runs GWG, the colour
+# kernel CWG.  One persistent wave of a kernel is SMs x warpgroups x samples per tile.
+def front_wgs(n_kpt):
+    return 2 if n_kpt <= 14 else 3 if n_kpt <= 20 else 2 if n_kpt <= 28 else 1
+
+
+TAIL_WGS = 2
+COLOUR_WGS = 3
+
+
+def tile_samples(n_views):
+    """Samples per tile of the geometry front kernel (two warps of 32 // n_views samples), the density tail and the colour
+    kernel (four warps)."""
+    return 2 * (32 // n_views), 64, 4 * (32 // n_views)
+
+
 def psnr(a, b):
     mse = float(np.mean((np.asarray(a, np.float64) - np.asarray(b, np.float64)) ** 2))
     return 99.0 if mse == 0 else 10.0 * np.log10(1.0 / mse)
