@@ -6,8 +6,8 @@
 // Three persistent kernels per batch of valid samples:
 //   geo_front_kernel  : gather + keypoint encoding + geometry MLP (L0-L3) + view pooling.  A row is one (sample, source view)
 //                       pair; the NV views of a sample sit in NV adjacent lanes (32 / NV samples per warp: 10 with 3 views,
-//                       8 with 4), so the pooling (reference src/utils.py:722-748) is an NV-lane shuffle.  Writes the pooled
-//                       [mean | var] (fp32) of every sample to a scratch buffer.
+//                       8 with 4).  The pooling (reference src/utils.py:722-748) reads the sample's NV rows from shared
+//                       memory and writes the pooled [mean | var] (fp32) of every sample to a scratch buffer.
 //   geo_tail_kernel   : density tail per sample (P0|compress, P1 with two-term fp16 weights W_hi + W_lo and two-term
 //                       activations, 64->2 head in fp32).  Writes alpha/sdf and, where a colour is needed, the 24-wide
 //                       compressed latent (fp16).  The tail is a kernel of its own because the geometry stages' W_hi tiles and
@@ -244,6 +244,40 @@ struct Group<3> {
   __device__ float vmax(float x) const { return fmaxf(x, fmaxf(__shfl_sync(FULL, x, l1), __shfl_sync(FULL, x, l2))); }
 };
 
+// Weighted mean and variance over the NV views of four feature columns (x[u]: view u's columns, w[u]: its weight), with the
+// roundings Group<NV>::sum gives the lane of view 0: mean = sum_u w_u x_u, var = sum_u (w_u dl_u) dl_u with dl_u = x_u - mean_u,
+// where mean_u is the mean as view u's lane sums it (with 3 views that lane starts at its own view, so the three means may
+// differ in the last bit).  The explicit _rn intrinsics keep ptxas from contracting any of it into an FFMA.
+template <int NV>
+__device__ __forceinline__ float pool_sum(const float* a, int u0) {
+  float s = a[u0];
+#pragma unroll
+  for (int i = 1; i < NV; ++i) s = __fadd_rn(s, a[(u0 + i) % NV]);
+  return s;
+}
+template <int NV>
+__device__ __forceinline__ void pool_views(const float* w, const float4* x, float4& mn, float4& vr) {
+  float m[4], q[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float xs[NV], p[NV], e[NV];
+#pragma unroll
+    for (int u = 0; u < NV; ++u) {
+      xs[u] = i == 0 ? x[u].x : i == 1 ? x[u].y : i == 2 ? x[u].z : x[u].w;
+      p[u] = __fmul_rn(w[u], xs[u]);
+    }
+    m[i] = pool_sum<NV>(p, 0);
+#pragma unroll
+    for (int u = 0; u < NV; ++u) {
+      const float dl = __fsub_rn(xs[u], NV == 3 ? pool_sum<NV>(p, u) : m[i]);
+      e[u] = __fmul_rn(__fmul_rn(w[u], dl), dl);
+    }
+    q[i] = pool_sum<NV>(e, 0);
+  }
+  mn = make_float4(m[0], m[1], m[2], m[3]);
+  vr = make_float4(q[0], q[1], q[2], q[3]);
+}
+
 // =====================================================================================================================
 // geometry front: stages L0-L3 + view pooling.  Warpgroup tile = 64 rows: row warps 0/1 hold rows 0-31 / 32-63 with
 // column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
@@ -259,7 +293,7 @@ constexpr long long POOL_SLICE = 1ll << 22;   // samples per front/tail launch p
 __host__ __device__ constexpr uint32_t front_tile_bytes(int n_kpt) {
   return 64u * (uint32_t)(tc_k0p(n_kpt) > 144 ? tc_k0p(n_kpt) : 144) * 2u;
 }
-static_assert(64 * D3S * 4 <= 64 * 144 * 2, "the L3 rows fit in the activation tile they replace");
+static_assert(64 * D3S * 4 + 64 * 4 <= 64 * 144 * 2, "the L3 rows and the rows' view weights fit in the activation tile");
 // Warpgroups per front CTA: as many tiles as fit beside the resident W_hi of stages 0..3 in the 227 KB an SM gives a block,
 // up to three.  The row threads' gathers are latency bound, so a third warpgroup helps hide them; the register file caps the
 // CTA at three (168 registers per thread at 384 threads).  Three tiles fit up to K0P 208 (20 keypoints: 223 232 B dynamic +
@@ -391,12 +425,12 @@ __device__ __forceinline__ void gather_feat8(const SceneS<NV>& S, int v, const P
 //                   load (the sample) instead of two dependent ones;
 //   FO_NEXT_SAMPLE  (with FO_NEXT_ID) the next tile's sample is also fetched, after L3, so a tile starts on no global load.
 // Each holds registers across the wgmma chain, and for some instantiations that makes ptxas serialise the chain's wgmma
-// instructions (warning C7511).  The table gives each instantiation the first of 7, 3, 6, 1, 2, 0 with which ptxas (CUDA 12.9,
-// -Xptxas -v) builds it without C7511 and without spills; every front instantiation compiles without C7511.  One digit per
+// instructions (warnings C7511 / C7520).  The table gives each instantiation the first of 7, 3, 6, 1, 2, 0 with which ptxas (CUDA
+// 12.9, -Xptxas -v) builds it without C7511, C7520 or spills; every front instantiation compiles without them.  One digit per
 // pair count NP = 1 .. 16.
 constexpr int FO_F8_EARLY = 1, FO_NEXT_ID = 2, FO_NEXT_SAMPLE = 4;
 __host__ __device__ constexpr int front_opts(int nv, int np, bool grid) {
-  const char* t = nv <= 3 ? (grid ? "3777716677777737" : "7773777731776337") : (grid ? "1736777767773766" : "7777777737777737");
+  const char* t = nv <= 3 ? (grid ? "3737777373777737" : "3737777776777377") : (grid ? "3776377777777736" : "7773777777777717");
   return t[np - 1] - '0';
 }
 
@@ -518,33 +552,32 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
       float dd[3];
       fetch_sample<GRID>(src, idn, pn, dd);
     }
-    // ---- L3 rows to shared memory (over the dead activation tile), then the view pooling: weighted mean || variance over
-    //      the NV lanes of the group (src/utils.py:722-748); this thread owns 32 of the 64 feature columns
+    // ---- L3 rows and the rows' view weights to shared memory (over the dead activation tile), then the view pooling: weighted
+    //      mean || variance over the NV rows of a sample (src/utils.py:722-748), one (sample, 4 columns) item per thread at a time
 #pragma unroll
     for (int m = 0; m < 16; ++m) {
       const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 8 * (m >> 1) + 2 * (lane & 3);
       *reinterpret_cast<float2*>(D3 + r * D3S + c) = make_float2(d[2 * m], d[2 * m + 1]);
     }
+    if (h == 0) D3[64 * D3S + row] = pw;
     tc::named_sync(bar_id, 128);
-    {
-      const bool writer = lane < NV * SPW && v == 0 && si < end;
-      float* out = pool + (si - base) * POOL_W + 32 * h;
-      const float* x = D3 + row * D3S + 32 * h;
+    for (int it = t & 127; it < FSPT * 16; it += 128) {
+      const int s = it >> 4, c = 4 * (it & 15);
+      const int r0 = (s / SPW) * 32 + NV * (s % SPW);   // row of the sample's view 0
+      float4 x[NV];
+      float w[NV];
 #pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4) {
-        const float4 xv = *reinterpret_cast<const float4*>(x + 4 * c4);
-        const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-        float mn[4], vr[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          mn[i] = grp.sum(pw * xs[i]);
-          const float dl = xs[i] - mn[i];
-          vr[i] = grp.sum(pw * dl * dl);
-        }
-        if (writer) {
-          *reinterpret_cast<float4*>(out + 4 * c4) = make_float4(mn[0], mn[1], mn[2], mn[3]);
-          *reinterpret_cast<float4*>(out + 64 + 4 * c4) = make_float4(vr[0], vr[1], vr[2], vr[3]);
-        }
+      for (int u = 0; u < NV; ++u) {
+        x[u] = *reinterpret_cast<const float4*>(D3 + (r0 + u) * D3S + c);
+        w[u] = D3[64 * D3S + r0 + u];
+      }
+      float4 mn, vr;
+      pool_views<NV>(w, x, mn, vr);
+      const long long sj = base + (long long)tile * FSPT + s;
+      if (sj < end) {
+        float* out = pool + (sj - base) * POOL_W + c;
+        *reinterpret_cast<float4*>(out) = mn;
+        *reinterpret_cast<float4*>(out + 64) = vr;
       }
     }
     tc::named_sync(bar_id, 128);   // the L3 rows are read: the next tile's input may overwrite them
