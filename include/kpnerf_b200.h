@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define KPN_ABI_VERSION 3
+#define KPN_ABI_VERSION 4
 #define KPN_MAX_VIEWS 4
 #define KPN_MAX_KPT 32
 #define KPN_NUM_LAYERS 19
@@ -129,6 +129,18 @@ typedef struct {
                                  serves both here) */
 } kpn_opts;
 
+/* An explicit batch of n rays (kpn_render_rays): any pixel subset, camera model or set of cameras.  Ray i marches the points
+ * origins[i] + z * dirs[i] for z in [near, far], where [near, far] is near_far[i] tightened to the scene's bounding box exactly as
+ * the lattice rays' are (reference src/model.py:1039-1043, 1178-1237, with the ray's own origin); dirs[i] is also the view
+ * direction of its samples. */
+typedef struct {
+  const float* origins;   /* (n,3) ray origins */
+  const float* dirs;      /* (n,3) unit directions, used as given (the library does not renormalise) */
+  const float* near_far;  /* (n,2) near/far distances along dirs BEFORE the bounding-box clip */
+  long long n;
+  int mem;                /* kpn_mem of the three arrays */
+} kpn_rays;
+
 /* Outputs of batch_render_pifu_nerf (reference src/model.py:1065-1096); any pointer may be NULL. */
 typedef struct {
   float* tex_fg;       /* (3,ny,nx) */
@@ -185,6 +197,20 @@ int kpn_set_scene(kpn_ctx* ctx, const kpn_scene* scene, void* stream);
 /* KeypointNeRF.batch_render_pifu_nerf, eval branch (reference src/model.py:942-1108);
  * with step=1 it renders what render_pifu_nerf assembles from stride^2 passes (src/model.py:897-940). */
 int kpn_render(kpn_ctx* ctx, const kpn_target* target, const kpn_opts* opts, const kpn_out* out, void* stream);
+
+/* The eval branch of batch_render_pifu_nerf (reference src/model.py:1038-1096) on the explicit rays of `rays` instead of a
+ * target's pixel lattice: the same coarse pass, fine pass, opts and debug outputs as kpn_render, with the kpn_out planes
+ * shaped as a lattice of nx = n, ny = 1 (tex_fg (3,n), depth / alpha / sdf (n), contrib (n,S_c), z_fine and
+ * z_fine_override (n,S_c+S_f)).  kpn_render_rays(kpn_camera_rays(T)[idx]) equals kpn_render(T) at the pixels idx bit for bit,
+ * for any subset, order or concatenation of cameras.  n == 0: KPN_OK, nothing is done; null arrays or n < 0: KPN_ERR_ARG;
+ * no scene: KPN_ERR_STATE; sample counts, engines and their refusals as kpn_render. */
+int kpn_render_rays(kpn_ctx* ctx, const kpn_rays* rays, const kpn_opts* opts, const kpn_out* out, void* stream);
+
+/* The rays kpn_render marches for the target's pixel lattice, pixel j*nx+i at index j*nx+i: origins (R,3) = -t^T R,
+ * dirs (R,3) = normalize(K^-1 [x,y,1] R), near_far (R,2) = |znear K^-1 [x,y,1]|, |zfar K^-1 [x,y,1]| (before the bounding-box
+ * clip), R = nx*ny.  Needs neither weights nor a scene.  `mem` = kpn_mem of the three outputs (the target's own mem field
+ * describes K and RT). */
+int kpn_camera_rays(kpn_ctx* ctx, const kpn_target* target, float* origins, float* dirs, float* near_far, int mem, void* stream);
 
 /* KeypointNeRF.query (reference src/model.py:690-782): pts, view (n,3) -> out5 (n,5) = [sdf_raw, rad, r, g, b],
  * valid (n) in {0,1}.  Rows with valid==0 carry out5 = [0,0,0,0,0] (the reference's values there are

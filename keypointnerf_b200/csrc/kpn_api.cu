@@ -70,9 +70,9 @@ struct kpn_ctx {
   DevBuf stage[4];             // host-sourced maps before packing
   DevBuf atlas[4];             // f64, f8, ftex, img (channel-last fp32)
   DevBuf atlas_fg;
-  // per-chunk workspace: rays (dir, near/far), per-ray list ranges of up to two segments, the work list, the compact per-sample
+  // per-chunk workspace: rays (origin, dir, near/far), per-ray list ranges of up to two segments, the work list, the compact per-sample
   // records (alpha+sdf, rgb, compositing weight), the fine depths, the colour kernel's latent scratch + work list
-  DevBuf ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
+  DevBuf ws_rayo, ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
   DevBuf ws_out, ws_in;
   // marching cubes: per-point vertex offsets, per-cell case bytes and face offsets, scan scratch; the state kpn_mesh_begin
   // leaves for kpn_mesh_emit
@@ -152,7 +152,7 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   for (auto& b : c->stage) b.release();
   for (auto& b : c->atlas) b.release();
   c->atlas_fg.release();
-  for (DevBuf* b : {&c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
+  for (DevBuf* b : {&c->ws_rayo, &c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
                     &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in, &c->mc_vofs, &c->mc_cases, &c->mc_tofs,
                     &c->mc_tmp})
     b->release();
@@ -468,8 +468,9 @@ static long long chunk_rays(long long R, int Smax) {
 // every per-chunk workspace buffer of a render of Rc rays x (Sc coarse, Smax total) samples
 static int reserve_render(kpn_ctx* c, long long Rc, int Sc, int Smax, bool fine, bool contrib, bool ert) {
   const size_t n = (size_t)Rc * Smax;
+  KPN_CUDA(c, c->ws_rayo.reserve((size_t)Rc * 3 * sizeof(float)));
   KPN_CUDA(c, c->ws_rayd.reserve((size_t)Rc * 3 * sizeof(float)));
-  KPN_CUDA(c, c->ws_raynf.reserve((size_t)Rc * 2 * sizeof(float)));
+  KPN_CUDA(c, c->ws_raynf.reserve((size_t)Rc * 4 * sizeof(float)));   // clipped near/far | a lattice's near/far before the clip
   KPN_CUDA(c, c->ws_rayseg.reserve((size_t)Rc * 4 * sizeof(int)));   // start | cnt of segment 0, start | cnt of segment 1
   KPN_CUDA(c, c->ws_list.reserve(n * sizeof(int)));
   KPN_CUDA(c, c->ws_ao.reserve(n * sizeof(float2)));
@@ -490,6 +491,7 @@ extern "C" int kpn_reserve(kpn_ctx* c, long long max_rays, int max_samples) {
   int rc = reserve_render(c, Rc, max_samples, max_samples, true, true, true);
   if (rc != KPN_OK) return rc;
   KPN_CUDA(c, c->ws_out.reserve((size_t)max_rays * 11 * sizeof(float)));   // host-output staging: 3+1+1+3+1+1+1 planes
+  KPN_CUDA(c, c->ws_in.reserve((size_t)max_rays * 8 * sizeof(float)));     // host-input staging of kpn_render_rays: o, d, near/far
   return KPN_OK;
 }
 
@@ -501,22 +503,8 @@ static int begin_counters(kpn_ctx* c, cudaStream_t st) {
   return KPN_OK;
 }
 
-extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, const kpn_out* out, void* stream) {
-  if (!c || !tg || !op || !out) return KPN_ERR_ARG;
-  DeviceGuard g(c->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_render");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
-  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
-  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
-  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
-  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
-  const long long R = (long long)tg->nx * tg->ny;
-  const int Smax = Sc + Sf;
-  if (R * Smax >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many samples");
-
-  // target camera -> device constants
+// Target camera -> device constants (d_target); with_scene: also the bound scene's foreground windows.
+static int upload_target(kpn_ctx* c, const kpn_target* tg, bool with_scene, cudaStream_t st) {
   cudaMemcpyKind kind = in_kind(tg->mem);
   KPN_CUDA(c, cudaMemcpyAsync(c->d_raw_target->K, tg->K, sizeof(float) * 16, kind, st));
   KPN_CUDA(c, cudaMemcpyAsync(c->d_raw_target->RT, tg->RT, sizeof(float) * 16, kind, st));
@@ -525,10 +513,25 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
   ht.znear = tg->znear; ht.zfar = tg->zfar; ht.x0 = tg->x0; ht.y0 = tg->y0; ht.step = tg->step; ht.nx = tg->nx; ht.ny = tg->ny;
   ht.step_y = tg->step_y > 0 ? tg->step_y : tg->step;
   KPN_CUDA(c, cudaMemcpyAsync(c->d_target, &ht, sizeof(ht), cudaMemcpyHostToDevice, st));
-  KPN_CUDA(c, launch_prep_target(c->d_raw_target, c->d_target, c->d_scene, st));
+  KPN_CUDA(c, launch_prep_target(c->d_raw_target, c->d_target, with_scene ? c->d_scene : nullptr, st));
   c->launches++;
-  const float* d_o = reinterpret_cast<const float*>(reinterpret_cast<const char*>(c->d_target) + offsetof(DevTarget, o));
+  return KPN_OK;
+}
 
+// The rays a render marches: the pixel lattice of the target in d_target (lattice), or explicit device arrays o, d (R,3) and
+// nf (R,2, near/far before the bounding-box clip).
+struct RaySource {
+  bool lattice;
+  const float* o;
+  const float* d;
+  const float* nf;
+};
+
+// The render of R rays x (S_c [+ S_f]) samples shared by kpn_render and kpn_render_rays: chunks of rays, each through the coarse
+// pass, the resampling and the fine pass; outputs are planes of R values (kpn_out).  Arguments are checked by the caller.
+static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn_opts* op, const kpn_out* out, cudaStream_t st) {
+  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
+  const int Smax = Sc + Sf;
   // outputs: render into device planes, copy to the host at the end if requested
   float* user[7] = {out->tex_fg, out->depth, out->alpha, out->tex_fg_fine, out->depth_fine, out->alpha_fine, out->sdf};
   const int planes[7] = {3, 1, 1, 3, 1, 1, 1};
@@ -558,6 +561,9 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
   int* list = c->ws_list.as<int>();
   float2* ao = c->ws_ao.as<float2>();
   float* rgbw = c->ws_rgb.as<float>();
+  const float* ro = nullptr;   // the current chunk's rays
+  const float* rd = nullptr;
+  const float* rnf = nullptr;
   // One pass over nr rays x S samples (zbuf == nullptr: the coarse pass, uniform depths): front (rays + validity + ray-ordered
   // work list) -> shading -> compositing.  Early-ray termination (ert_eps > 0, S >= 8): the front half of every ray is shaded
   // and composited first; rays whose transmittance behind it is < ert_eps get no entries for the back half (their remaining
@@ -567,7 +573,7 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
                   float* cw) -> int {
     SampleSrc src;
     memset(&src, 0, sizeof(src));
-    src.mode = 0; src.S = S; src.ray_d = c->ws_rayd.as<float>(); src.z = zbuf; src.ray_nf = c->ws_raynf.as<float>(); src.o = d_o;
+    src.mode = 0; src.S = S; src.ray_d = rd; src.z = zbuf; src.ray_nf = c->ws_raynf.as<float>(); src.o = ro;
     const long long n = (long long)nr * S;
     int* start0 = seg; int* cnt0 = seg + Rc; int* start1 = seg + 2 * Rc; int* cnt1 = seg + 3 * Rc;
     const bool two = ert_on && S >= 8;
@@ -575,8 +581,8 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
     ShadeOut so;
     memset(&so, 0, sizeof(so));
     so.ao = ao; so.rgb = rgbw;
-    KPN_CUDA(c, launch_front(c->d_scene, c->d_target, r0, nr, S, zbuf, c->ws_rayd.as<float>(), c->ws_raynf.as<float>(), list, 0,
-                             c->d_counters + slot, start0, cnt0, two ? ErtSegment{0, half, nullptr, 0.0f} : ErtSegment{0, 0, nullptr, 0.0f}, st));
+    KPN_CUDA(c, launch_front(c->d_scene, c->d_target, nr, S, zbuf, ro, rd, rnf, c->ws_raynf.as<float>(), list, 0, c->d_counters + slot,
+                             start0, cnt0, two ? ErtSegment{0, half, nullptr, 0.0f} : ErtSegment{0, 0, nullptr, 0.0f}, st));
     c->launches++;
     so.list_base = 0;
     int r1 = shade_batch(c, src, list, c->d_counters + slot, c->d_counters2 + slot, two ? (long long)nr * half : n, 0, so, op->engine, st);
@@ -585,8 +591,8 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
       KPN_CUDA(c, launch_composite(list, ao, rgbw, start0, cnt0, nullptr, nullptr, zbuf, c->ws_raynf.as<float>(), r0, nr, S, R, nullptr,
                                    nullptr, nullptr, nullptr, c->ws_ert.as<float>(), nullptr, st));
       const int base1 = nr * half;
-      KPN_CUDA(c, launch_front(c->d_scene, c->d_target, r0, nr, S, zbuf ? zbuf : nullptr, c->ws_rayd.as<float>(), c->ws_raynf.as<float>(),
-                               list, base1, c->d_counters + slot + 1, start1, cnt1, ErtSegment{half, S, c->ws_ert.as<float>(), op->ert_eps}, st));
+      KPN_CUDA(c, launch_front(c->d_scene, c->d_target, nr, S, zbuf, ro, rd, rnf, c->ws_raynf.as<float>(), list, base1,
+                               c->d_counters + slot + 1, start1, cnt1, ErtSegment{half, S, c->ws_ert.as<float>(), op->ert_eps}, st));
       c->launches += 2;
       so.list_base = base1;
       r1 = shade_batch(c, src, list + base1, c->d_counters + slot + 1, c->d_counters2 + slot + 1, n - base1, 0, so, op->engine, st);
@@ -601,6 +607,13 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
   for (long long ch = 0; ch < nchunks; ++ch) {
     const long long r0 = ch * Rc;
     const int nr = (int)((R - r0) < Rc ? (R - r0) : Rc);
+    if (rays.lattice) {
+      ro = c->ws_rayo.as<float>(); rd = c->ws_rayd.as<float>(); rnf = c->ws_raynf.as<float>() + 2 * Rc;
+      KPN_CUDA(c, launch_camera_rays(c->d_target, r0, nr, c->ws_rayo.as<float>(), c->ws_rayd.as<float>(), c->ws_raynf.as<float>() + 2 * Rc, st));
+      c->launches++;
+    } else {
+      ro = rays.o + 3 * r0; rd = rays.d + 3 * r0; rnf = rays.nf + 2 * r0;
+    }
     // coarse pass; with early-ray termination its weights must still cover every sample of the ray for the resampling pass:
     // rays that terminated early simply have zero weight behind the cut
     rc = pass((int)r0, nr, Sc, nullptr, (int)(4 * ch), dev[0], dev[1], dev[2], nullptr, need_contrib ? c->ws_cw.as<float>() : nullptr);
@@ -636,6 +649,83 @@ extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, 
       if (user[i]) KPN_CUDA(c, cudaMemcpyAsync(user[i], dev[i], (size_t)planes[i] * R * sizeof(float), cudaMemcpyDeviceToHost, st));
   }
   return wd_snapshot(c, st);
+}
+
+
+extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, const kpn_out* out, void* stream) {
+  if (!c || !tg || !op || !out) return KPN_ERR_ARG;
+  DeviceGuard g(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_render");
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
+  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
+  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
+  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
+  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
+  const long long R = (long long)tg->nx * tg->ny;
+  if (R * (Sc + Sf) >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many samples");
+  int rc = upload_target(c, tg, true, st);
+  if (rc != KPN_OK) return rc;
+  return render_rays(c, R, RaySource{true, nullptr, nullptr, nullptr}, op, out, st);
+}
+
+extern "C" int kpn_render_rays(kpn_ctx* c, const kpn_rays* rays, const kpn_opts* op, const kpn_out* out, void* stream) {
+  if (!c || !rays || !op || !out || rays->n < 0) return KPN_ERR_ARG;
+  if (rays->n == 0) return KPN_OK;
+  DeviceGuard g(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!rays->origins || !rays->dirs || !rays->near_far) KPN_FAIL(c, KPN_ERR_ARG, "null ray arrays");
+  if (rays->mem != KPN_MEM_HOST && rays->mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_render_rays");
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
+  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
+  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
+  const long long R = rays->n;
+  if (R > 0x7fffffffll || R * (Sc + Sf) >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many rays / samples (%lld rays)", R);
+  RaySource src{false, rays->origins, rays->dirs, rays->near_far};
+  if (rays->mem == KPN_MEM_HOST) {   // staged like kpn_query's inputs: o | d | near/far
+    const size_t b3 = (size_t)R * 3 * sizeof(float), b2 = (size_t)R * 2 * sizeof(float);
+    KPN_CUDA(c, c->ws_in.reserve(2 * b3 + b2));
+    char* b = c->ws_in.as<char>();
+    KPN_CUDA(c, cudaMemcpyAsync(b, rays->origins, b3, cudaMemcpyHostToDevice, st));
+    KPN_CUDA(c, cudaMemcpyAsync(b + b3, rays->dirs, b3, cudaMemcpyHostToDevice, st));
+    KPN_CUDA(c, cudaMemcpyAsync(b + 2 * b3, rays->near_far, b2, cudaMemcpyHostToDevice, st));
+    src.o = reinterpret_cast<const float*>(b); src.d = reinterpret_cast<const float*>(b + b3);
+    src.nf = reinterpret_cast<const float*>(b + 2 * b3);
+  }
+  KPN_CUDA(c, launch_prep_target(nullptr, c->d_target, c->d_scene, st));   // the scene's foreground windows only
+  c->launches++;
+  return render_rays(c, R, src, op, out, st);
+}
+
+extern "C" int kpn_camera_rays(kpn_ctx* c, const kpn_target* tg, float* origins, float* dirs, float* near_far, int mem, void* stream) {
+  if (!c || !tg || !origins || !dirs || !near_far) return KPN_ERR_ARG;
+  DeviceGuard g(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
+  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
+  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  const long long R = (long long)tg->nx * tg->ny;
+  int rc = upload_target(c, tg, false, st);
+  if (rc != KPN_OK) return rc;
+  float* o = origins; float* d = dirs; float* nf = near_far;
+  const size_t b3 = (size_t)R * 3 * sizeof(float), b2 = (size_t)R * 2 * sizeof(float);
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, c->ws_out.reserve(2 * b3 + b2));
+    o = c->ws_out.as<float>(); d = reinterpret_cast<float*>(c->ws_out.as<char>() + b3);
+    nf = reinterpret_cast<float*>(c->ws_out.as<char>() + 2 * b3);
+  }
+  KPN_CUDA(c, launch_camera_rays(c->d_target, 0, R, o, d, nf, st));
+  c->launches++;
+  if (mem == KPN_MEM_HOST) {
+    KPN_CUDA(c, cudaMemcpyAsync(origins, o, b3, cudaMemcpyDeviceToHost, st));
+    KPN_CUDA(c, cudaMemcpyAsync(dirs, d, b3, cudaMemcpyDeviceToHost, st));
+    KPN_CUDA(c, cudaMemcpyAsync(near_far, nf, b2, cudaMemcpyDeviceToHost, st));
+  }
+  return KPN_OK;
 }
 
 extern "C" int kpn_query(kpn_ctx* c, const float* pts, const float* view, int n, float* out5, uint8_t* valid, int mem,

@@ -44,7 +44,8 @@ __device__ __forceinline__ void fetch_sample(const SampleSrc& src, long long id,
     float z = sample_depth(src, id, r);
     d[0] = src.ray_d[3 * r + 0]; d[1] = src.ray_d[3 * r + 1]; d[2] = src.ray_d[3 * r + 2];
     // eval_pts = cam_pos + cam_rays * z  (reference src/model.py:1057)
-    p[0] = src.o[0] + d[0] * z; p[1] = src.o[1] + d[1] * z; p[2] = src.o[2] + d[2] * z;
+    const float* o = src.o + 3 * r;
+    p[0] = o[0] + d[0] * z; p[1] = o[1] + d[1] * z; p[2] = o[2] + d[2] * z;
   } else {
     p[0] = src.pts[3 * id + 0]; p[1] = src.pts[3 * id + 1]; p[2] = src.pts[3 * id + 2];
     d[0] = src.view[3 * id + 0]; d[1] = src.view[3 * id + 1]; d[2] = src.view[3 * id + 2];

@@ -3,8 +3,9 @@
 // Stages (reference src/model.py:1018-1096 for the eval branch of batch_render_pifu_nerf):
 //   pack_nhwc      feature maps NCHW -> channel-last atlases (once per scene)
 //   prep_*         derived camera constants on device (no host sync)
-//   front          one kernel per pass: pixel lattice -> ray (direction, near/far incl. bbox clip), depths, per-sample validity
-//                  (frustum + foreground in every view), ray-ordered compacted work list
+//   camera_rays    pixel lattice -> rays (origin, direction, near/far before the bbox clip)
+//   front          one kernel per pass: rays -> bbox clip, depths, per-sample validity (frustum + foreground in every view),
+//                  ray-ordered compacted work list
 //   compact        the same validity test + compaction for explicit points (KeypointNeRF.query)
 //   shade_simt     per-sample gather + keypoint encoding + MLPs for tiles of 64 valid samples
 //   composite      alpha compositing along the ray over the compact per-sample records
@@ -119,9 +120,12 @@ __device__ void fg_windows(const DevScene& sc, float win[MAXV][4]) {
   }
 }
 
+// raw: the target camera (nullptr: leave the camera fields alone); sc: the bound scene whose foreground windows ray_interval
+// reads (nullptr: no scene, the windows are left alone).
 __global__ void prep_target_kernel(const RawTarget* __restrict__ raw, DevTarget* tg, const DevScene* __restrict__ sc) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  fg_windows(*sc, tg->win);
+  if (sc) fg_windows(*sc, tg->win);
+  if (!raw) return;
   double a[9], inv[9];
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) a[i * 3 + j] = (double)raw->K[i * 4 + j];
@@ -139,8 +143,9 @@ __global__ void prep_target_kernel(const RawTarget* __restrict__ raw, DevTarget*
 // ------------------------------------------------------------------------------------------------
 // rays (reference src/model.py:1018-1043, 1178-1237)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ray_for_pixel(const DevScene& sc, const DevTarget& tg, float px, float py,
-                                              float d[3], float& n_r, float& f_r) {
+// The ray of lattice pixel (px, py): origin, unit direction and the near/far distances of the znear / zfar planes along it,
+// before the bounding-box clip (reference src/model.py:1026-1036).
+__device__ __forceinline__ void camera_ray(const DevTarget& tg, float px, float py, float o[3], float d[3], float& n_r, float& f_r) {
   const float* iK = tg.invK;
   float dc[3], gn[3], gf[3];
   for (int i = 0; i < 3; ++i) {
@@ -154,7 +159,12 @@ __device__ __forceinline__ void ray_for_pixel(const DevScene& sc, const DevTarge
   for (int j = 0; j < 3; ++j) w[j] = dc[0] * tg.R[j] + dc[1] * tg.R[3 + j] + dc[2] * tg.R[6 + j];
   float nn = fmaxf(sqrtf(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]), 1e-12f);
   d[0] = w[0] / nn; d[1] = w[1] / nn; d[2] = w[2] / nn;
-  // bbox slab test with the "exactly two face hits" rule
+  o[0] = tg.o[0]; o[1] = tg.o[1]; o[2] = tg.o[2];
+}
+
+// Tightens a ray's near/far to its bounding-box interval: slab test with the "exactly two face hits" rule, from the ray's own
+// origin (reference src/model.py:1039-1043, 1178-1237).
+__device__ __forceinline__ void bbox_clip(const DevScene& sc, const float o[3], const float d[3], float& n_r, float& f_r) {
   float dd[3];
   for (int i = 0; i < 3; ++i) dd[i] = fabsf(d[i]) < 1e-5f ? 1e-5f : d[i];
   float ddn = sqrtf(dd[0] * dd[0] + dd[1] * dd[1] + dd[2] * dd[2]);
@@ -164,12 +174,12 @@ __device__ __forceinline__ void ray_for_pixel(const DevScene& sc, const DevTarge
   float tn = 3.0e38f, tf = -3.0e38f;
   for (int f = 0; f < 6; ++f) {
     int ax = f % 3;
-    float t = (b[f] - tg.o[ax]) / dd[ax];
-    float p[3] = {t * dd[0] + tg.o[0], t * dd[1] + tg.o[1], t * dd[2] + tg.o[2]};
+    float t = (b[f] - o[ax]) / dd[ax];
+    float p[3] = {t * dd[0] + o[0], t * dd[1] + o[1], t * dd[2] + o[2]};
     bool in = p[0] >= b[0] - eps && p[0] <= b[3] + eps && p[1] >= b[1] - eps && p[1] <= b[4] + eps &&
               p[2] >= b[2] - eps && p[2] <= b[5] + eps;
     if (in) {
-      float e[3] = {p[0] - tg.o[0], p[1] - tg.o[1], p[2] - tg.o[2]};
+      float e[3] = {p[0] - o[0], p[1] - o[1], p[2] - o[2]};
       float dist = sqrtf(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]) / ddn;
       tn = fminf(tn, dist); tf = fmaxf(tf, dist);
       ++cnt;
@@ -180,12 +190,30 @@ __device__ __forceinline__ void ray_for_pixel(const DevScene& sc, const DevTarge
   if (hit && tf < f_r) f_r = tf;
 }
 
+// Rays of lattice pixels r0 .. r0 + n - 1 (pixel r = j*nx + i): o, d (n,3), near/far (n,2) before the bounding-box clip.  One
+// thread per ray and no loop: a grid-stride loop lets the compiler hoist the loop-invariant products (iK[.][2] * znear, ...) out of
+// it, and a product hoisted out of the block of its sum is no longer fused into an FMA, which changes the rays' last bits.
+__global__ void camera_rays_kernel(const DevTarget* __restrict__ tgp, long long r0, long long n, float* __restrict__ o,
+                                   float* __restrict__ d, float* __restrict__ nf) {
+  const DevTarget& tg = *tgp;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long r = r0 + i;
+  const int ix = (int)(r % tg.nx), iy = (int)(r / tg.nx);
+  float oo[3], dd[3], n_r, f_r;
+  camera_ray(tg, (float)(tg.x0 + tg.step * ix), (float)(tg.y0 + tg.step_y * iy), oo, dd, n_r, f_r);
+  o[3 * i + 0] = oo[0]; o[3 * i + 1] = oo[1]; o[3 * i + 2] = oo[2];
+  d[3 * i + 0] = dd[0]; d[3 * i + 1] = dd[1]; d[3 * i + 2] = dd[2];
+  nf[2 * i + 0] = n_r; nf[2 * i + 1] = f_r;
+}
+
 // ------------------------------------------------------------------------------------------------
 // front end of a render pass: rays + depths + validity + ray-ordered compaction in ONE kernel
 // ------------------------------------------------------------------------------------------------
-// One warp per ray, 8 rays per block iteration.  Coarse pass (zbuf == nullptr): the warp derives the ray (direction, near/far
-// incl. the bbox clip) and stores it; its depths are the uniform ones and are never stored (every consumer recomputes them
-// with coarse_depth()).  Fine pass: the ray is re-read and the depths come from zbuf (R, S).  Lane l tests samples l, l+32, ..
+// One warp per ray, 8 rays per block iteration.  The chunk's rays come in as origins / directions (ray_o, ray_d) and, for the
+// coarse pass (zbuf == nullptr), near/far before the bounding-box clip (nf_in): the warp clips them with the ray's own origin
+// and stores the clipped near/far in ray_nf; the coarse depths are the uniform ones and are never stored (every consumer
+// recomputes them with coarse_depth()).  Fine pass: the depths come from zbuf (R, S).  Lane l tests samples l, l+32, ..
 // (3 projections + frustum + foreground lookups, reference src/model.py:713-739); the ballots give the ray's valid samples in
 // order.  The 8 rays of a block iteration reserve ONE contiguous range of the work list with one atomicAdd; inside it the
 // entries are ordered by (ray, sample), so that ray r owns list[ray_start[r] .. +ray_cnt[r]) -- the compositing pass walks
@@ -233,11 +261,11 @@ constexpr int FRONT_THREADS = FRONT_WARPS * 32;
 constexpr int FRONT_MASKW = 2048;   // ballot words of one batch of rays held in shared memory (8 KB)
 constexpr int FRONT_MAXW = 40;      // ballot words per ray: up to 1280 samples (256 coarse + 1024 fine)
 
-struct FrontRay { float d[3], n, f, zlo, zhi; int wa, wb; };   // per ray of a batch: direction, near/far, interval, word range
+struct FrontRay { float o[3], d[3], n, f, zlo, zhi; int wa, wb; };   // per ray of a batch: origin, direction, near/far, interval, word range
 
 __global__ void __launch_bounds__(FRONT_THREADS, 4)
-front_kernel(const DevScene* __restrict__ scp, const DevTarget* __restrict__ tgp, int r0, int nr, int S,
-             const float* __restrict__ zbuf, float* __restrict__ ray_d, float* __restrict__ ray_nf,
+front_kernel(const DevScene* __restrict__ scp, const DevTarget* __restrict__ tgp, int nr, int S, const float* __restrict__ zbuf,
+             const float* __restrict__ ray_o, const float* __restrict__ ray_d, const float* __restrict__ nf_in, float* __restrict__ ray_nf,
              int* __restrict__ list, int list_base, int* __restrict__ counter, int* __restrict__ ray_start,
              int* __restrict__ ray_cnt, ErtSegment ert) {
   const DevScene& sc = *scp;
@@ -252,27 +280,24 @@ front_kernel(const DevScene* __restrict__ scp, const DevTarget* __restrict__ tgp
   // rays per batch: as many as a block has threads, fewer when their ballot words would not fit (very long rays)
   const int batch = min(FRONT_THREADS, (FRONT_MASKW / nwords) & ~31);
   const int s_lo = ert.s_hi > 0 ? ert.s_lo : 0, s_hi = ert.s_hi > 0 ? ert.s_hi : S;
-  const float o0 = tg.o[0], o1 = tg.o[1], o2 = tg.o[2];
   for (int base = blockIdx.x * batch; base < nr; base += gridDim.x * batch) {   // block-uniform trip count
-    // ---- phase A, one THREAD per ray: the ray, its near/far, the depth interval outside of which nothing can be valid, and the
+    // ---- phase A, one THREAD per ray: the ray, its clipped near/far, the depth interval outside of which nothing can be valid, and the
     //      range of 32-sample words that can intersect it (uniform depths are monotone in the sample index)
     if (threadIdx.x < batch) {
       const int i = base + threadIdx.x;
       FrontRay fr;
       fr.wa = 0; fr.wb = 0;
       if (i < nr) {
+        fr.o[0] = ray_o[3 * i + 0]; fr.o[1] = ray_o[3 * i + 1]; fr.o[2] = ray_o[3 * i + 2];
+        fr.d[0] = ray_d[3 * i + 0]; fr.d[1] = ray_d[3 * i + 1]; fr.d[2] = ray_d[3 * i + 2];
         if (zbuf == nullptr) {
-          const int r = r0 + i;
-          const int ix = r % tg.nx, iy = r / tg.nx;
-          ray_for_pixel(sc, tg, (float)(tg.x0 + tg.step * ix), (float)(tg.y0 + tg.step_y * iy), fr.d, fr.n, fr.f);
-          ray_d[3 * i + 0] = fr.d[0]; ray_d[3 * i + 1] = fr.d[1]; ray_d[3 * i + 2] = fr.d[2];
+          fr.n = nf_in[2 * i + 0]; fr.f = nf_in[2 * i + 1];
+          bbox_clip(sc, fr.o, fr.d, fr.n, fr.f);
           ray_nf[2 * i + 0] = fr.n; ray_nf[2 * i + 1] = fr.f;
         } else {
-          fr.d[0] = ray_d[3 * i + 0]; fr.d[1] = ray_d[3 * i + 1]; fr.d[2] = ray_d[3 * i + 2];
           fr.n = 0.0f; fr.f = 0.0f;
         }
-        const float oo[3] = {o0, o1, o2};
-        ray_interval(sc, tg, oo, fr.d, fr.zlo, fr.zhi);
+        ray_interval(sc, tg, fr.o, fr.d, fr.zlo, fr.zhi);
         const bool dead = ert.ray_alpha != nullptr && 1.0f - ert.ray_alpha[i] < ert.eps;   // ray already opaque
         if (!dead && fr.zlo <= fr.zhi) {
           int sa = s_lo, sb = s_hi;
@@ -308,7 +333,7 @@ front_kernel(const DevScene* __restrict__ scp, const DevTarget* __restrict__ tgp
           if (s < S && s >= s_lo && s < s_hi) {
             const float z = zbuf ? zbuf[(long long)i * S + s] : coarse_depth(fr.n, fr.f, s, S);
             if (z >= fr.zlo && z <= fr.zhi) {   // outside the ray's interval no view can accept the sample
-              const float p[3] = {o0 + fr.d[0] * z, o1 + fr.d[1] * z, o2 + fr.d[2] * z};   // reference src/model.py:1057
+              const float p[3] = {fr.o[0] + fr.d[0] * z, fr.o[1] + fr.d[1] * z, fr.o[2] + fr.d[2] * z};   // reference src/model.py:1057
               Proj q[MAXV];
               ok = sample_valid(sc, p, q);
             }
@@ -950,9 +975,14 @@ cudaError_t launch_prep_target(const RawTarget* raw, DevTarget* tg, const DevSce
   prep_target_kernel<<<1, 32, 0, st>>>(raw, tg, sc);
   return cudaGetLastError();
 }
-cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr, int S, const float* zbuf, float* ray_d,
-                         float* ray_nf, int* list, int list_base, int* counter, int* ray_start, int* ray_cnt, const ErtSegment& ert,
-                         cudaStream_t st) {
+cudaError_t launch_camera_rays(const DevTarget* tg, long long r0, long long n, float* o, float* d, float* nf, cudaStream_t st) {
+  if (n < 1) return cudaSuccess;
+  camera_rays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(tg, r0, n, o, d, nf);
+  return cudaGetLastError();
+}
+cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int nr, int S, const float* zbuf, const float* ray_o,
+                         const float* ray_d, const float* nf_in, float* ray_nf, int* list, int list_base, int* counter, int* ray_start,
+                         int* ray_cnt, const ErtSegment& ert, cudaStream_t st) {
   // persistent grid: as many blocks as are resident at once (no partial second wave)
   static std::atomic<int> per_sm{0};
   int bps = per_sm.load(std::memory_order_acquire);
@@ -965,8 +995,8 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int nwords = (S + 31) / 32;
   const int batch = std::min(FRONT_THREADS, (FRONT_MASKW / nwords) & ~31);
-  front_kernel<<<grid_for(nr, batch, sms * bps), FRONT_THREADS, 0, st>>>(sc, tg, r0, nr, S, zbuf, ray_d, ray_nf, list, list_base,
-                                                                            counter, ray_start, ray_cnt, ert);
+  front_kernel<<<grid_for(nr, batch, sms * bps), FRONT_THREADS, 0, st>>>(sc, tg, nr, S, zbuf, ray_o, ray_d, nf_in, ray_nf, list,
+                                                                            list_base, counter, ray_start, ray_cnt, ert);
   return cudaGetLastError();
 }
 cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out, int out_w,

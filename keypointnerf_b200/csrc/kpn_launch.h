@@ -9,9 +9,13 @@ cudaError_t launch_pack_nhwc_f32(const float* in, float* out, int V, int C, int 
 cudaError_t launch_prep_scene(const RawScene* raw, DevScene* sc, cudaStream_t st);
 cudaError_t launch_fg_box(DevScene* sc, int n_views, cudaStream_t st);
 cudaError_t launch_prep_target(const RawTarget* raw, DevTarget* tg, const DevScene* sc, cudaStream_t st);
-cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int r0, int nr, int S, const float* zbuf, float* ray_d,
-                         float* ray_nf, int* list, int list_base, int* counter, int* ray_start, int* ray_cnt, const ErtSegment& ert,
-                         cudaStream_t st);
+// rays of lattice pixels r0 .. r0 + n - 1 of the target: o, d (n,3), near/far before the bounding-box clip (n,2)
+cudaError_t launch_camera_rays(const DevTarget* tg, long long r0, long long n, float* o, float* d, float* nf, cudaStream_t st);
+// ray_o, ray_d (nr,3): the chunk's rays; nf_in (nr,2): their near/far before the clip (coarse pass, zbuf == nullptr; may alias
+// nothing the kernel writes); ray_nf (nr,2): the clipped near/far (written by the coarse pass)
+cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int nr, int S, const float* zbuf, const float* ray_o,
+                         const float* ray_d, const float* nf_in, float* ray_nf, int* list, int list_base, int* counter, int* ray_start,
+                         int* ray_cnt, const ErtSegment& ert, cudaStream_t st);
 cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out, int out_w,
                            uint8_t* valid_out, cudaStream_t st);
 cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,

@@ -430,7 +430,7 @@ __device__ __forceinline__ void gather_feat8(const SceneS<NV>& S, int v, const P
 // pair count NP = 1 .. 16.
 constexpr int FO_F8_EARLY = 1, FO_NEXT_ID = 2, FO_NEXT_SAMPLE = 4;
 __host__ __device__ constexpr int front_opts(int nv, int np, bool grid) {
-  const char* t = nv <= 3 ? (grid ? "3737777373777737" : "3737777776777377") : (grid ? "3776377777777736" : "7773777777777717");
+  const char* t = nv <= 3 ? (grid ? "7726777776337767" : "1733777773773717") : (grid ? "7777776777333771" : "7777773777173373");
   return t[np - 1] - '0';
 }
 

@@ -53,7 +53,7 @@ struct DevScene {
 struct DevTarget {
   float invK[9];           // inverse(K[:3,:3]) (src/model.py:1031)
   float R[9];
-  float o[3];              // camera centre -t^T R (src/model.py:1036)
+  float o[3];              // camera centre -t^T R (src/model.py:1036): the origin of every lattice ray
   float znear, zfar;
   int x0, y0, step, nx, ny;
   int step_y;              // lattice step along y (== step for the reference's square lattices)
@@ -72,7 +72,7 @@ struct DevWeightsF32 {
 // Where the samples of a shading launch come from.  The grid fields of mode 2 share storage with the pointers, which that mode
 // does not read, so that the struct (a kernel parameter of every shading kernel) keeps the layout of modes 0 and 1.
 struct SampleSrc {
-  int mode;            // 0: rays (p = o + d*z(ray, i)),  1: explicit points,  2: grid points (no view direction)
+  int mode;            // 0: rays (p = o(ray) + d(ray)*z(ray, i)),  1: explicit points,  2: grid points (no view direction)
   int S;               // samples per ray (mode 0)
   union {
     struct {
@@ -81,7 +81,7 @@ struct SampleSrc {
       const float* ray_nf; // (R,2) near/far along the ray (used when z == nullptr)
       const float* pts;    // (n,3)   (mode 1)
       const float* view;   // (n,3)   (mode 1)
-      const float* o;      // (3) ray origin on device (mode 0)
+      const float* o;      // (R,3) ray origins (mode 0)
     };
     struct {
       float g_org[3], g_sp[3];   // grid origin and spacing (mode 2): p[a] = g_org[a] + g_sp[a] * idx_a, no FMA contraction

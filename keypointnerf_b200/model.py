@@ -435,11 +435,8 @@ class KeypointNeRF(nn.Module):
                                     sp_data, out_device=None, **config)
 
     @staticmethod
-    def _render(net, img_in, cam_in, cam_tar, step, x_off, y_off, tar_img, feat_geo, feat_tex, sp_data, out_device,
-                **config):
-        S_c = config.get("sample_per_ray_c", 64)
-        S_f = config.get("sample_per_ray_f", 64)
-        fine = config.get("fine", False)
+    def _check_config(config):
+        """The eval-branch options this build renders; the training-time ones raise."""
         if not config.get("uniform", False):
             raise NotImplementedError("uniform=False (stratified jitter of the sample depths, the default of dr_kwargs in "
                                       "configs/zju.json) is a training-time option outside this build: pass uniform=True, as the "
@@ -450,6 +447,14 @@ class KeypointNeRF(nn.Module):
             raise NotImplementedError("rand_noise_std > 0 (density noise, dr_kwargs.rand_noise_std of configs/zju.json) is a "
                                       "training-time option outside this build: the reference's render callers do not pass it "
                                       "(src/model.py:453-473)")
+
+    @staticmethod
+    def _render(net, img_in, cam_in, cam_tar, step, x_off, y_off, tar_img, feat_geo, feat_tex, sp_data, out_device,
+                **config):
+        S_c = config.get("sample_per_ray_c", 64)
+        S_f = config.get("sample_per_ray_f", 64)
+        fine = config.get("fine", False)
+        KeypointNeRF._check_config(config)
         width = int(cam_tar.get("width", cam_in["width"]))
         height = int(cam_tar.get("height", cam_in["height"]))
         znear = cam_tar.get("znear", cam_in["znear"])
@@ -474,3 +479,27 @@ class KeypointNeRF(nn.Module):
                     msk = config["msk"].reshape(1, 1, height, width)
                     out["tar_alpha"] = msk[:, :, ys][:, :, :, xs].float().to(out["tex_fg"].device)
         return out
+
+    # ---- explicit rays (the eval branch of src/model.py:1038-1096 on given rays) ------------------------------------------
+    @staticmethod
+    def render_rays(net, img_in, cam_in, rays_o, rays_d, near_far, sp_data={}, **config):
+        """Render explicit rays: ``rays_o``, ``rays_d`` (n,3) (unit directions, used as given) and ``near_far`` (n,2) (before the
+        clip to ``config["bounds"]``), e.g. the pixels of a ``mask_at_box``, an orthographic bundle or the rays of several
+        cameras at once.  Same ``**config`` keys as ``render_pifu_nerf``.  Returns ``tex_fg`` (3,n), ``depth`` / ``alpha`` (n,)
+        (and with ``fine``: ``tex_fg_fine``, ``depth_fine``, ``alpha_fine``, ``sdf``) on the rays' device; ray i equals the
+        pixel of ``render_pifu_nerf`` whose ray it is, bit for bit."""
+        config = dict(config)
+        feat_geo = config.pop("feat_geo", None)
+        feat_tex = config.pop("feat_tex", None)
+        KeypointNeRF._check_config(config)
+        if feat_geo is None:
+            feat_geo = net.attach_geo_feat(img_in, return_val=True)
+        if feat_tex is None:
+            feat_tex = net.attach_tex_feat(img_in, return_val=True)
+        fine = config.get("fine", False)
+        m = net._bind_scene(cam_in, feat_geo, feat_tex, sp_data, img_in, config.get("src_foreground_mask"), config["bounds"])
+        res = m.render_rays(rays_o, rays_d, near_far, S_c=config.get("sample_per_ray_c", 64), S_f=config.get("sample_per_ray_f", 64),
+                            fine=fine, engine=net.engine, ert_eps=config.get("ert_eps", 0.0),
+                            out_device="cuda" if rays_o.is_cuda else "cpu")
+        keys = ["tex_fg", "depth", "alpha"] + (["tex_fg_fine", "depth_fine", "alpha_fine", "sdf"] if fine else [])
+        return {k: res[k] for k in keys}

@@ -146,56 +146,103 @@ class RayMarcher:
         """Raise if a tensor-core kernel's barrier wait gave up since the last check (``kpn_check_health``)."""
         L.check(self.lib, self.ctx, self.lib.kpn_check_health(self.ctx, self._stream()), "kpn_check_health")
 
-    def render(self, *, K, RT, znear, zfar, x0, y0, step, nx, ny, S_c, S_f=0, fine=False, out_device=None,
-               engine=0, z_fine_override=None, debug=False, ert_eps=0.0, step_y=0) -> dict:
-        """One ``kpn_render`` call.  Returns planar tensors on ``out_device`` ('cuda' or 'cpu';
-        default: where K lives)."""
+    @staticmethod
+    def _target(K, RT, znear, zfar, x0, y0, step, nx, ny, step_y):
         K, RT = _f32c(K).reshape(-1, 4, 4)[0].contiguous(), _f32c(RT).reshape(-1, 4, 4)[0].contiguous()
         if RT.device != K.device:
             RT = RT.to(K.device)
-        if out_device is None:
-            out_device = "cuda" if K.is_cuda else "cpu"
         tg = L.KpnTarget()
         tg.K, tg.RT = K.data_ptr(), RT.data_ptr()
         tg.znear, tg.zfar = float(znear), float(zfar)
         tg.x0, tg.y0, tg.step, tg.nx, tg.ny, tg.step_y = int(x0), int(y0), int(step), int(nx), int(ny), int(step_y)
         tg.mem = L.KPN_MEM_DEVICE if K.is_cuda else L.KPN_MEM_HOST
+        return tg, [K, RT]
+
+    def _march(self, call, what, shape, out_device, S_c, S_f, fine, engine, z_fine_override, debug, ert_eps, keep) -> dict:
+        """One kpn_render / kpn_render_rays call ``call(opts, out)`` whose rays form an image of ``shape`` ((ny, nx) or (n,))."""
         op = L.KpnOpts()
         op.sample_per_ray_c, op.sample_per_ray_f, op.fine = int(S_c), int(S_f), int(bool(fine))
         op.ert_eps, op.engine = float(ert_eps), int(engine)
         host_out = str(out_device).startswith("cpu")
         odev = torch.device("cpu") if host_out else torch.device("cuda", self.device)
+        n = int(np.prod(shape))
 
         def alloc(*shape):
             if host_out:   # fresh host tensors per call, like the reference's .cpu() (src/model.py:929)
                 return torch.empty(*shape, dtype=torch.float32, pin_memory=_PINNED_OUT)
             return torch.empty(*shape, dtype=torch.float32, device=odev)
 
-        res = {"tex_fg": alloc(3, ny, nx), "depth": alloc(ny, nx), "alpha": alloc(ny, nx)}
+        res = {"tex_fg": alloc(3, *shape), "depth": alloc(*shape), "alpha": alloc(*shape)}
         if fine:
-            res.update({"tex_fg_fine": alloc(3, ny, nx), "depth_fine": alloc(ny, nx), "alpha_fine": alloc(ny, nx),
-                        "sdf": alloc(ny, nx)})
+            res.update({"tex_fg_fine": alloc(3, *shape), "depth_fine": alloc(*shape), "alpha_fine": alloc(*shape),
+                        "sdf": alloc(*shape)})
             if debug:
-                res["z_fine"] = alloc(ny * nx, S_c + S_f)
+                res["z_fine"] = alloc(n, S_c + S_f)
         if debug:
-            res["contrib"] = alloc(ny * nx, S_c)
-        keep = [K, RT]
+            res["contrib"] = alloc(n, S_c)
         if z_fine_override is not None:
             zo = _f32c(z_fine_override).to(odev).contiguous()
-            assert zo.numel() == nx * ny * (S_c + S_f)
+            assert zo.numel() == n * (S_c + S_f)
             op.z_fine_override = zo.data_ptr()
             keep.append(zo)
         out = L.KpnOut()
         for k, v in res.items():
             setattr(out, k, v.data_ptr())
         out.mem = L.KPN_MEM_HOST if host_out else L.KPN_MEM_DEVICE
-        L.check(self.lib, self.ctx,
-                self.lib.kpn_render(self.ctx, C.byref(tg), C.byref(op), C.byref(out), self._stream()), "kpn_render")
+        L.check(self.lib, self.ctx, call(C.byref(op), C.byref(out)), what)
         self._keep_call = keep
         if host_out:  # results are host tensors: make them readable on return (reference does .cpu(), src/model.py:929)
             torch.cuda.current_stream(self.device).synchronize()
             self.check_health()   # the watchdog words travelled with the results: a tripped barrier wait raises here
         return res
+
+    def render(self, *, K, RT, znear, zfar, x0, y0, step, nx, ny, S_c, S_f=0, fine=False, out_device=None,
+               engine=0, z_fine_override=None, debug=False, ert_eps=0.0, step_y=0) -> dict:
+        """One ``kpn_render`` call.  Returns planar tensors on ``out_device`` ('cuda' or 'cpu';
+        default: where K lives)."""
+        tg, keep = self._target(K, RT, znear, zfar, x0, y0, step, nx, ny, step_y)
+        if out_device is None:
+            out_device = "cuda" if keep[0].is_cuda else "cpu"
+        call = lambda op, out: self.lib.kpn_render(self.ctx, C.byref(tg), op, out, self._stream())
+        return self._march(call, "kpn_render", (ny, nx), out_device, S_c, S_f, fine, engine, z_fine_override, debug, ert_eps, keep)
+
+    def camera_rays(self, *, K, RT, znear, zfar, x0=0, y0=0, step=1, nx, ny, step_y=0):
+        """The rays ``render`` marches for the same lattice (``kpn_camera_rays``): ``(origins (n,3), dirs (n,3), near_far (n,2))``
+        on K's device, ray ``j*nx + i`` for pixel (i, j), near/far before the bounding-box clip.  Needs no weights or scene."""
+        tg, keep = self._target(K, RT, znear, zfar, x0, y0, step, nx, ny, step_y)
+        n = int(nx) * int(ny)
+        on_dev = keep[0].is_cuda
+        kw = dict(device=keep[0].device) if on_dev else dict(pin_memory=True)
+        o = torch.empty(n, 3, dtype=torch.float32, **kw)
+        d = torch.empty(n, 3, dtype=torch.float32, **kw)
+        nf = torch.empty(n, 2, dtype=torch.float32, **kw)
+        L.check(self.lib, self.ctx,
+                self.lib.kpn_camera_rays(self.ctx, C.byref(tg), o.data_ptr(), d.data_ptr(), nf.data_ptr(),
+                                         L.KPN_MEM_DEVICE if on_dev else L.KPN_MEM_HOST, self._stream()), "kpn_camera_rays")
+        self._keep_call = keep
+        if not on_dev:
+            torch.cuda.current_stream(self.device).synchronize()
+        return o, d, nf
+
+    def render_rays(self, origins, dirs, near_far, *, S_c, S_f=0, fine=False, engine=0, ert_eps=0.0, out_device=None,
+                    z_fine_override=None, debug=False) -> dict:
+        """One ``kpn_render_rays`` call on explicit rays: ``origins``, ``dirs`` (n,3) (unit directions, used as given),
+        ``near_far`` (n,2) before the bounding-box clip.  Returns the dict of ``render`` with every (ny, nx) plane shaped (n,),
+        on ``out_device`` (default: where ``origins`` lives)."""
+        o = _f32c(origins).reshape(-1, 3)
+        d, nf = _f32c(dirs).reshape(-1, 3), _f32c(near_far).reshape(-1, 2)
+        d, nf = d.to(o.device).contiguous(), nf.to(o.device).contiguous()
+        n = o.shape[0]
+        if d.shape[0] != n or nf.shape[0] != n:
+            raise ValueError(f"render_rays: {n} origins, {d.shape[0]} directions, {nf.shape[0]} near/far pairs")
+        if out_device is None:
+            out_device = "cuda" if o.is_cuda else "cpu"
+        rays = L.KpnRays()
+        rays.origins, rays.dirs, rays.near_far, rays.n = o.data_ptr(), d.data_ptr(), nf.data_ptr(), n
+        rays.mem = L.KPN_MEM_DEVICE if o.is_cuda else L.KPN_MEM_HOST
+        call = lambda op, out: self.lib.kpn_render_rays(self.ctx, C.byref(rays), op, out, self._stream())
+        return self._march(call, "kpn_render_rays", (n,), out_device, S_c, S_f, fine, engine, z_fine_override, debug, ert_eps,
+                           [o, d, nf])
 
     def query(self, pts: torch.Tensor, view: torch.Tensor, engine: int = 0):
         """``KeypointNeRF.query`` for explicit points: returns out (n,5)=[sdf_raw, rad, r, g, b], valid (n,) bool."""
