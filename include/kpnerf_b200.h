@@ -195,7 +195,8 @@ int kpn_set_weights(kpn_ctx* ctx, const kpn_weights* w);
 int kpn_set_scene(kpn_ctx* ctx, const kpn_scene* scene, void* stream);
 
 /* KeypointNeRF.batch_render_pifu_nerf, eval branch (reference src/model.py:942-1108);
- * with step=1 it renders what render_pifu_nerf assembles from stride^2 passes (src/model.py:897-940). */
+ * with step=1 it renders what render_pifu_nerf assembles from stride^2 passes (src/model.py:897-940).
+ * A lattice of more than 2^31 - 1 rays (nx*ny) is refused with KPN_ERR_ARG, as is a kpn_render_rays batch of more. */
 int kpn_render(kpn_ctx* ctx, const kpn_target* target, const kpn_opts* opts, const kpn_out* out, void* stream);
 
 /* The eval branch of batch_render_pifu_nerf (reference src/model.py:1038-1096) on the explicit rays of `rays` instead of a

@@ -104,6 +104,51 @@ struct kpn_ctx {
     if (_e != cudaSuccess) KPN_FAIL(ctx, KPN_ERR_CUDA, "%s: %s", #expr, cudaGetErrorString(_e)); \
   } while (0)
 
+#define KPN_TRY(expr)                  \
+  do {                                 \
+    int _rc = (expr);                  \
+    if (_rc != KPN_OK) return _rc;     \
+  } while (0)
+
+static bool mem_ok(int mem) { return mem == KPN_MEM_HOST || mem == KPN_MEM_DEVICE; }
+
+// The host arrays of one call, staged in one device buffer: ws_in for inputs (stage() copies them in), ws_out for outputs
+// (unstage() copies them back), so that a call's inputs and outputs never alias.  Every staged array gets the slice at the next
+// 256-byte boundary.  stage() reserves the buffer once, for the whole layout, before any copy into it: DevBuf::reserve frees the
+// old allocation when it grows.
+struct Staging {
+  DevBuf* buf;
+  bool in, host;   // inputs (ws_in) or outputs (ws_out); the call's arrays are in host memory (KPN_MEM_HOST)
+  int n = 0;
+  void* ptr[8];
+  size_t bytes[8], off[8], total = 0;
+  Staging(kpn_ctx* c, bool in, bool host) : buf(in ? &c->ws_in : &c->ws_out), in(in), host(host) {}
+  // array p of b bytes: staged when it is a host array, or when `scratch` (the call needs the buffer even if p == nullptr)
+  int add(const void* p, size_t b, bool scratch = false) {
+    ptr[n] = const_cast<void*>(p);
+    bytes[n] = (host && p) || scratch ? b : 0;
+    off[n] = total;
+    total += (bytes[n] + 255) / 256 * 256;
+    return n++;
+  }
+  // the device pointer the call uses for array i: its slice when staged, else the caller's own pointer
+  template <typename T> T* dev(int i) const {
+    return static_cast<T*>(bytes[i] ? static_cast<void*>(buf->as<char>() + off[i]) : ptr[i]);
+  }
+};
+
+static int stage(kpn_ctx* c, const Staging& s, cudaStream_t st) {
+  KPN_CUDA(c, s.buf->reserve(s.total));
+  for (int i = 0; s.in && i < s.n; ++i)
+    if (s.bytes[i] && s.ptr[i]) KPN_CUDA(c, cudaMemcpyAsync(s.dev<void>(i), s.ptr[i], s.bytes[i], cudaMemcpyHostToDevice, st));
+  return KPN_OK;
+}
+static int unstage(kpn_ctx* c, const Staging& s, cudaStream_t st) {
+  for (int i = 0; i < s.n; ++i)
+    if (s.bytes[i] && s.ptr[i]) KPN_CUDA(c, cudaMemcpyAsync(s.ptr[i], s.dev<void>(i), s.bytes[i], cudaMemcpyDeviceToHost, st));
+  return KPN_OK;
+}
+
 extern "C" int kpn_abi_version(void) { return KPN_ABI_VERSION; }
 
 extern "C" int kpn_create(int device, kpn_ctx** out) {
@@ -163,6 +208,21 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
 
 extern "C" const char* kpn_last_error(const kpn_ctx* c) { return c ? c->err.c_str() : "null context"; }
 
+// Stream-ordered copy of every module's watchdog words into out (TC_WD_MODULES x TC_WD_WORDS), and their reset.
+static int wd_read(kpn_ctx* c, unsigned int* out, cudaStream_t st) {
+  void* w[TC_WD_MODULES];
+  KPN_CUDA(c, tc_watchdog_words(w));
+  for (int m = 0; m < TC_WD_MODULES; ++m)
+    KPN_CUDA(c, cudaMemcpyAsync(out + TC_WD_WORDS * m, w[m], TC_WD_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  return KPN_OK;
+}
+static int wd_clear(kpn_ctx* c, cudaStream_t st) {
+  void* w[TC_WD_MODULES];
+  KPN_CUDA(c, tc_watchdog_words(w));
+  for (int m = 0; m < TC_WD_MODULES; ++m) KPN_CUDA(c, cudaMemsetAsync(w[m], 0, TC_WD_WORDS * sizeof(unsigned int), st));
+  return KPN_OK;
+}
+
 // Device watchdog (kpn_tc.cuh): a barrier wait that gives up raises a sticky device flag; every later wait of every later
 // tensor-core launch then aborts after a few polls, i.e. the engine keeps producing garbage until the flag is cleared.  Every
 // render/query ends with an asynchronous copy of the flag words into pinned host memory (wd_snapshot); every entry point starts
@@ -177,15 +237,12 @@ static int wd_check(kpn_ctx* c, cudaStream_t st) {
   if (!w) return KPN_OK;
   const unsigned int blk = w[1], thr = w[2], tag = w[3], par = w[4];
   for (int i = 0; i < TC_WD_MODULES * TC_WD_WORDS; ++i) c->h_wd[i] = 0u;
-  KPN_CUDA(c, tc_watchdog_clear_async(st));
+  KPN_TRY(wd_clear(c, st));
   KPN_FAIL(c, KPN_ERR_CUDA, "device watchdog: a barrier wait of a tensor-core kernel gave up (block %u, thread %u, tag 0x%x, parity %u); "
            "the results of that call (and of tensor-core calls enqueued after it) are invalid; the flag has been cleared",
            blk, thr, tag, par);
 }
-static int wd_snapshot(kpn_ctx* c, cudaStream_t st) {
-  KPN_CUDA(c, tc_watchdog_read_async(c->h_wd, st));
-  return KPN_OK;
-}
+static int wd_snapshot(kpn_ctx* c, cudaStream_t st) { return wd_read(c, c->h_wd, st); }
 
 extern "C" int kpn_check_health(kpn_ctx* c, void* stream) {
   if (!c) return KPN_ERR_ARG;
@@ -337,7 +394,7 @@ extern "C" int kpn_set_scene(kpn_ctx* c, const kpn_scene* s, void* stream) {
   DeviceGuard g(c->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (!c->have_weights) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_weights must precede kpn_set_scene");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  KPN_TRY(wd_check(c, st));
   if (s->n_views < 1 || s->n_views > KPN_MAX_VIEWS)
     KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "n_views=%d unsupported (1..%d)", s->n_views, KPN_MAX_VIEWS);
   if (s->n_kpt != c->n_kpt) KPN_FAIL(c, KPN_ERR_ARG, "scene n_kpt=%d != weights n_kpt=%d", s->n_kpt, c->n_kpt);
@@ -345,7 +402,7 @@ extern "C" int kpn_set_scene(kpn_ctx* c, const kpn_scene* s, void* stream) {
     KPN_FAIL(c, KPN_ERR_ARG, "null scene pointer");
   if (s->f64_c != 64 || s->f8_c != 8 || s->ftex_c != 8)
     KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "feature channels (%d,%d,%d) != (64,8,8)", s->f64_c, s->f8_c, s->ftex_c);
-  if (s->mem != KPN_MEM_HOST && s->mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!mem_ok(s->mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
   const int V = s->n_views;
   cudaMemcpyKind kind = in_kind(s->mem);
 
@@ -435,17 +492,17 @@ static int shade_batch(kpn_ctx* c, const SampleSrc& src, const int* list, const 
     KPN_CUDA(c, c->ws_lat.reserve((size_t)n * 48));
     KPN_CUDA(c, c->ws_list2.reserve((size_t)n * 8));
     KPN_CUDA(c, c->ws_pool.reserve(tc_pool_bytes(n)));
-    int launches = 0;
-    KPN_CUDA(c, launch_shade_tc(c->d_scene, c->scene_views, c->tcc, c->wblob.as<uint8_t>(), c->wlo.as<uint8_t>(), engine == 2 ? 0 : 1, c->n_kpt, src,
-                                list, counter, n, query_mode, so, c->ws_lat.p, c->ws_pool.p, c->ws_list2.p, counter2, c->num_sms, em,
-                                &launches, st));
-    c->launches += launches;
   }
-  else {
-    KPN_CUDA(c, launch_shade_simt(c->d_scene, c->scene_views, c->d_wf32, src, list, counter, n, query_mode, so, c->num_sms, st));
-    if (c->profiling) KPN_CUDA(c, cudaEventRecord(em, st));
-    c->launches++;
-  }
+  ShadeBatch b;
+  b.sc = c->d_scene; b.n_views = c->scene_views; b.n_kpt = c->n_kpt;
+  b.src = src; b.list = list; b.counter = counter; b.n_max = n; b.query_mode = query_mode; b.so = so;
+  b.num_sms = c->num_sms; b.st = st;
+  b.wf32 = c->d_wf32;
+  b.tcc = &c->tcc; b.wblob = c->wblob.as<uint8_t>(); b.wlo = c->wlo.as<uint8_t>();
+  b.lo_mask = engine == 2 ? 0xC0 : 0xF0;   // single-term weights (engine 2) keep the A_lo passes only
+  b.lat = c->ws_lat.as<uint4>(); b.pool = c->ws_pool.as<float>(); b.list2 = c->ws_list2.as<int2>(); b.count2 = counter2;
+  b.after_geo = em; b.launches = &c->launches;
+  KPN_CUDA(c, use_tc ? launch_shade_tc(b) : launch_shade_simt(b));
   if (c->profiling) KPN_CUDA(c, cudaEventRecord(e1, st));
   return KPN_OK;
 }
@@ -484,14 +541,25 @@ static int reserve_render(kpn_ctx* c, long long Rc, int Sc, int Smax, bool fine,
   return KPN_OK;
 }
 
+constexpr int OUT_W[7] = {3, 1, 1, 3, 1, 1, 1};   // floats per ray of the kpn_out planes tex_fg .. sdf
+constexpr int RAY_W[3] = {3, 3, 2};               // floats per ray of origins, dirs, near/far
+
+// The staging of n per-ray float arrays of R rays, a[i] with w[i] floats per ray: a render's kpn_out planes, kpn_render_rays'
+// inputs, kpn_camera_rays' outputs.  a == nullptr: room for every array, the most a render stages.
+static Staging ray_planes(kpn_ctx* c, bool in, bool host, long long R, int n, const int* w, const float* const* a) {
+  Staging s(c, in, host);
+  for (int i = 0; i < n; ++i) s.add(a ? a[i] : nullptr, (size_t)w[i] * R * sizeof(float), !a);
+  return s;
+}
+
 extern "C" int kpn_reserve(kpn_ctx* c, long long max_rays, int max_samples) {
   if (!c || max_rays < 1 || max_samples < 1) return KPN_ERR_ARG;
   DeviceGuard g(c->device);
   const long long Rc = chunk_rays(max_rays, max_samples);
-  int rc = reserve_render(c, Rc, max_samples, max_samples, true, true, true);
-  if (rc != KPN_OK) return rc;
-  KPN_CUDA(c, c->ws_out.reserve((size_t)max_rays * 11 * sizeof(float)));   // host-output staging: 3+1+1+3+1+1+1 planes
-  KPN_CUDA(c, c->ws_in.reserve((size_t)max_rays * 8 * sizeof(float)));     // host-input staging of kpn_render_rays: o, d, near/far
+  KPN_TRY(reserve_render(c, Rc, max_samples, max_samples, true, true, true));
+  // the host staging of the outputs and of kpn_render_rays' inputs, laid out as a render lays them out
+  KPN_CUDA(c, c->ws_out.reserve(ray_planes(c, false, true, max_rays, 7, OUT_W, nullptr).total));
+  KPN_CUDA(c, c->ws_in.reserve(ray_planes(c, true, true, max_rays, 3, RAY_W, nullptr).total));
   return KPN_OK;
 }
 
@@ -533,29 +601,20 @@ static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn
   const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
   const int Smax = Sc + Sf;
   // outputs: render into device planes, copy to the host at the end if requested
-  float* user[7] = {out->tex_fg, out->depth, out->alpha, out->tex_fg_fine, out->depth_fine, out->alpha_fine, out->sdf};
-  const int planes[7] = {3, 1, 1, 3, 1, 1, 1};
-  float* dev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  const float* user[7] = {out->tex_fg, out->depth, out->alpha, out->tex_fg_fine, out->depth_fine, out->alpha_fine, out->sdf};
   const bool host_out = out->mem == KPN_MEM_HOST;
-  if (host_out) {
-    size_t tot = 0;
-    for (int i = 0; i < 7; ++i) if (user[i]) tot += (size_t)planes[i] * R;
-    KPN_CUDA(c, c->ws_out.reserve(tot * sizeof(float)));
-    size_t off = 0;
-    for (int i = 0; i < 7; ++i) if (user[i]) { dev[i] = c->ws_out.as<float>() + off; off += (size_t)planes[i] * R; }
-  } else {
-    for (int i = 0; i < 7; ++i) dev[i] = user[i];
-  }
+  const Staging outs = ray_planes(c, false, host_out, R, 7, OUT_W, user);
+  KPN_TRY(stage(c, outs, st));
+  float* dev[7];
+  for (int i = 0; i < 7; ++i) dev[i] = outs.dev<float>(i);
 
   const long long Rc = chunk_rays(R, Smax);
   const long long nchunks = (R + Rc - 1) / Rc;
   if (nchunks * 4 > MAX_CHUNKS) KPN_FAIL(c, KPN_ERR_ARG, "frame too large for one call (%lld chunks)", nchunks);
   const bool need_contrib = op->fine || out->contrib;
   const bool ert_on = op->ert_eps > 0.0f;
-  int rc = reserve_render(c, Rc, Sc, Smax, op->fine != 0, need_contrib, ert_on);
-  if (rc != KPN_OK) return rc;
-  rc = begin_counters(c, st);
-  if (rc != KPN_OK) return rc;
+  KPN_TRY(reserve_render(c, Rc, Sc, Smax, op->fine != 0, need_contrib, ert_on));
+  KPN_TRY(begin_counters(c, st));
   cudaMemcpyKind okind = host_out ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
   int* seg = c->ws_rayseg.as<int>();
   int* list = c->ws_list.as<int>();
@@ -585,8 +644,7 @@ static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn
                              start0, cnt0, two ? ErtSegment{0, half, nullptr, 0.0f} : ErtSegment{0, 0, nullptr, 0.0f}, st));
     c->launches++;
     so.list_base = 0;
-    int r1 = shade_batch(c, src, list, c->d_counters + slot, c->d_counters2 + slot, two ? (long long)nr * half : n, 0, so, op->engine, st);
-    if (r1 != KPN_OK) return r1;
+    KPN_TRY(shade_batch(c, src, list, c->d_counters + slot, c->d_counters2 + slot, two ? (long long)nr * half : n, 0, so, op->engine, st));
     if (two) {
       KPN_CUDA(c, launch_composite(list, ao, rgbw, start0, cnt0, nullptr, nullptr, zbuf, c->ws_raynf.as<float>(), r0, nr, S, R, nullptr,
                                    nullptr, nullptr, nullptr, c->ws_ert.as<float>(), nullptr, st));
@@ -595,8 +653,7 @@ static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn
                                c->d_counters + slot + 1, start1, cnt1, ErtSegment{half, S, c->ws_ert.as<float>(), op->ert_eps}, st));
       c->launches += 2;
       so.list_base = base1;
-      r1 = shade_batch(c, src, list + base1, c->d_counters + slot + 1, c->d_counters2 + slot + 1, n - base1, 0, so, op->engine, st);
-      if (r1 != KPN_OK) return r1;
+      KPN_TRY(shade_batch(c, src, list + base1, c->d_counters + slot + 1, c->d_counters2 + slot + 1, n - base1, 0, so, op->engine, st));
     }
     KPN_CUDA(c, launch_composite(list, ao, rgbw, start0, cnt0, two ? start1 : nullptr, two ? cnt1 : nullptr, zbuf, c->ws_raynf.as<float>(),
                                  r0, nr, S, R, color, depth, alpha, sdf, nullptr, cw, st));
@@ -616,8 +673,7 @@ static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn
     }
     // coarse pass; with early-ray termination its weights must still cover every sample of the ray for the resampling pass:
     // rays that terminated early simply have zero weight behind the cut
-    rc = pass((int)r0, nr, Sc, nullptr, (int)(4 * ch), dev[0], dev[1], dev[2], nullptr, need_contrib ? c->ws_cw.as<float>() : nullptr);
-    if (rc != KPN_OK) return rc;
+    KPN_TRY(pass((int)r0, nr, Sc, nullptr, (int)(4 * ch), dev[0], dev[1], dev[2], nullptr, need_contrib ? c->ws_cw.as<float>() : nullptr));
     c->last_total += (unsigned long long)nr * Sc;
     if (need_contrib) {
       // dense weights (debug output) and / or the resampled + merged depths of the fine pass, one warp per ray
@@ -636,37 +692,46 @@ static int render_rays(kpn_ctx* c, long long R, const RaySource& rays, const kpn
       if (op->z_fine_override)
         KPN_CUDA(c, cudaMemcpyAsync(c->ws_zfine.p, op->z_fine_override + r0 * Smax, (size_t)nr * Smax * sizeof(float),
                                     in_kind(out->mem), st));
-      rc = pass((int)r0, nr, Smax, c->ws_zfine.as<float>(), (int)(4 * ch + 2), dev[3], dev[4], dev[5], dev[6], nullptr);
-      if (rc != KPN_OK) return rc;
+      KPN_TRY(pass((int)r0, nr, Smax, c->ws_zfine.as<float>(), (int)(4 * ch + 2), dev[3], dev[4], dev[5], dev[6], nullptr));
       c->last_total += (unsigned long long)nr * Smax;
       if (out->z_fine)
         KPN_CUDA(c, cudaMemcpyAsync(out->z_fine + r0 * Smax, c->ws_zfine.p, (size_t)nr * Smax * sizeof(float), okind, st));
     }
   }
   c->counters_used = (int)(4 * nchunks);
-  if (host_out) {
-    for (int i = 0; i < 7; ++i)
-      if (user[i]) KPN_CUDA(c, cudaMemcpyAsync(user[i], dev[i], (size_t)planes[i] * R * sizeof(float), cudaMemcpyDeviceToHost, st));
-  }
+  KPN_TRY(unstage(c, outs, st));
   return wd_snapshot(c, st);
 }
 
+
+static int check_target(kpn_ctx* c, const kpn_target* tg) {
+  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
+  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
+  return KPN_OK;
+}
+
+// The options and limits of a render of R rays, shared by kpn_render (tg: its target, whose lattice is checked here too) and
+// kpn_render_rays (tg == nullptr): the sample counts, at most 2^31 - 1 rays (the compositing kernel indexes the output planes
+// with an int) and 2^40 samples, and the memory kinds of the target and the outputs.
+static int check_render(kpn_ctx* c, const kpn_opts* op, const kpn_target* tg, long long R, const kpn_out* out) {
+  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
+  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
+  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
+  if (tg) KPN_TRY(check_target(c, tg));
+  if (R > 0x7fffffffll || R * (Sc + Sf) >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many rays / samples (%lld rays)", R);
+  if (!mem_ok(out->mem) || (tg && !mem_ok(tg->mem))) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  return KPN_OK;
+}
 
 extern "C" int kpn_render(kpn_ctx* c, const kpn_target* tg, const kpn_opts* op, const kpn_out* out, void* stream) {
   if (!c || !tg || !op || !out) return KPN_ERR_ARG;
   DeviceGuard g(c->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_render");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
-  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
-  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
-  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
-  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
+  KPN_TRY(wd_check(c, st));
   const long long R = (long long)tg->nx * tg->ny;
-  if (R * (Sc + Sf) >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many samples");
-  int rc = upload_target(c, tg, true, st);
-  if (rc != KPN_OK) return rc;
+  KPN_TRY(check_render(c, op, tg, R, out));
+  KPN_TRY(upload_target(c, tg, true, st));
   return render_rays(c, R, RaySource{true, nullptr, nullptr, nullptr}, op, out, st);
 }
 
@@ -676,56 +741,70 @@ extern "C" int kpn_render_rays(kpn_ctx* c, const kpn_rays* rays, const kpn_opts*
   DeviceGuard g(c->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (!rays->origins || !rays->dirs || !rays->near_far) KPN_FAIL(c, KPN_ERR_ARG, "null ray arrays");
-  if (rays->mem != KPN_MEM_HOST && rays->mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!mem_ok(rays->mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
   if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_render_rays");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
-  if (Sc < 1 || Sc > max_coarse_samples()) KPN_FAIL(c, KPN_ERR_ARG, "sample_per_ray_c=%d out of range", Sc);
-  if (op->fine && (Sc < 3 || Sf < 1 || Sf > 1024)) KPN_FAIL(c, KPN_ERR_ARG, "fine pass needs S_c>=3 and 1<=S_f<=1024");
+  KPN_TRY(wd_check(c, st));
   const long long R = rays->n;
-  if (R > 0x7fffffffll || R * (Sc + Sf) >= (1ll << 40)) KPN_FAIL(c, KPN_ERR_ARG, "too many rays / samples (%lld rays)", R);
-  RaySource src{false, rays->origins, rays->dirs, rays->near_far};
-  if (rays->mem == KPN_MEM_HOST) {   // staged like kpn_query's inputs: o | d | near/far
-    const size_t b3 = (size_t)R * 3 * sizeof(float), b2 = (size_t)R * 2 * sizeof(float);
-    KPN_CUDA(c, c->ws_in.reserve(2 * b3 + b2));
-    char* b = c->ws_in.as<char>();
-    KPN_CUDA(c, cudaMemcpyAsync(b, rays->origins, b3, cudaMemcpyHostToDevice, st));
-    KPN_CUDA(c, cudaMemcpyAsync(b + b3, rays->dirs, b3, cudaMemcpyHostToDevice, st));
-    KPN_CUDA(c, cudaMemcpyAsync(b + 2 * b3, rays->near_far, b2, cudaMemcpyHostToDevice, st));
-    src.o = reinterpret_cast<const float*>(b); src.d = reinterpret_cast<const float*>(b + b3);
-    src.nf = reinterpret_cast<const float*>(b + 2 * b3);
-  }
+  KPN_TRY(check_render(c, op, nullptr, R, out));
+  const float* a[3] = {rays->origins, rays->dirs, rays->near_far};
+  const Staging in = ray_planes(c, true, rays->mem == KPN_MEM_HOST, R, 3, RAY_W, a);
+  KPN_TRY(stage(c, in, st));
   KPN_CUDA(c, launch_prep_target(nullptr, c->d_target, c->d_scene, st));   // the scene's foreground windows only
   c->launches++;
-  return render_rays(c, R, src, op, out, st);
+  return render_rays(c, R, RaySource{false, in.dev<const float>(0), in.dev<const float>(1), in.dev<const float>(2)}, op, out, st);
 }
 
 extern "C" int kpn_camera_rays(kpn_ctx* c, const kpn_target* tg, float* origins, float* dirs, float* near_far, int mem, void* stream) {
   if (!c || !tg || !origins || !dirs || !near_far) return KPN_ERR_ARG;
   DeviceGuard g(c->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (tg->nx < 1 || tg->ny < 1 || tg->step < 1 || tg->step_y < 0) KPN_FAIL(c, KPN_ERR_ARG, "empty pixel lattice");
-  if (!tg->K || !tg->RT) KPN_FAIL(c, KPN_ERR_ARG, "null target camera");
-  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  KPN_TRY(check_target(c, tg));
+  if (!mem_ok(mem) || !mem_ok(tg->mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  KPN_TRY(wd_check(c, st));
   const long long R = (long long)tg->nx * tg->ny;
-  int rc = upload_target(c, tg, false, st);
-  if (rc != KPN_OK) return rc;
-  float* o = origins; float* d = dirs; float* nf = near_far;
-  const size_t b3 = (size_t)R * 3 * sizeof(float), b2 = (size_t)R * 2 * sizeof(float);
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, c->ws_out.reserve(2 * b3 + b2));
-    o = c->ws_out.as<float>(); d = reinterpret_cast<float*>(c->ws_out.as<char>() + b3);
-    nf = reinterpret_cast<float*>(c->ws_out.as<char>() + 2 * b3);
-  }
-  KPN_CUDA(c, launch_camera_rays(c->d_target, 0, R, o, d, nf, st));
+  KPN_TRY(upload_target(c, tg, false, st));
+  const float* a[3] = {origins, dirs, near_far};
+  const Staging outs = ray_planes(c, false, mem == KPN_MEM_HOST, R, 3, RAY_W, a);
+  KPN_TRY(stage(c, outs, st));
+  KPN_CUDA(c, launch_camera_rays(c->d_target, 0, R, outs.dev<float>(0), outs.dev<float>(1), outs.dev<float>(2), st));
   c->launches++;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, cudaMemcpyAsync(origins, o, b3, cudaMemcpyDeviceToHost, st));
-    KPN_CUDA(c, cudaMemcpyAsync(dirs, d, b3, cudaMemcpyDeviceToHost, st));
-    KPN_CUDA(c, cudaMemcpyAsync(near_far, nf, b2, cudaMemcpyDeviceToHost, st));
+  return unstage(c, outs, st);
+}
+
+// The point query shared by kpn_query (query_mode 1: base.pts, base.view) and kpn_query_grid (query_mode 2: the grid of base):
+// n points in chunks of 4 Mi, out_w floats per point into out and the validity mask into valid (may be nullptr), both of
+// kpn_mem `mem`.  Arguments are checked by the caller.
+static int query_points(kpn_ctx* c, const SampleSrc& base, long long n, float* out, int out_w, int query_mode, int mem,
+                        uint8_t* valid, const kpn_opts* op, cudaStream_t st) {
+  KPN_TRY(begin_counters(c, st));
+  if (n == 0) return KPN_OK;
+  Staging outs(c, false, mem == KPN_MEM_HOST);
+  outs.add(out, (size_t)n * out_w * sizeof(float));
+  outs.add(valid, (size_t)n, !valid);   // the compaction writes a mask whether or not the caller wants one
+  KPN_TRY(stage(c, outs, st));
+  float* dout = outs.dev<float>(0);
+  uint8_t* dvalid = outs.dev<uint8_t>(1);
+  const long long chunk = 4ll << 20;
+  const long long nchunks = (n + chunk - 1) / chunk;
+  if (nchunks > MAX_CHUNKS) KPN_FAIL(c, KPN_ERR_ARG, "too many points");
+  for (long long ch = 0; ch < nchunks; ++ch) {
+    const long long off = ch * chunk;
+    const long long m = (n - off) < chunk ? (n - off) : chunk;
+    SampleSrc src = base;
+    if (query_mode == 1) { src.pts += 3 * off; src.view += 3 * off; }
+    else src.g_id0 = off;
+    KPN_CUDA(c, c->ws_list.reserve((size_t)m * sizeof(int)));
+    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + out_w * off, out_w, dvalid + off, st));
+    c->launches++;
+    ShadeOut so;
+    memset(&so, 0, sizeof(so));
+    (query_mode == 1 ? so.out5 : so.out2) = dout + out_w * off;
+    KPN_TRY(shade_batch(c, src, c->ws_list.as<int>(), c->d_counters + ch, c->d_counters2 + ch, m, query_mode, so, op ? op->engine : 0, st));
   }
-  return KPN_OK;
+  c->counters_used = (int)nchunks;
+  c->last_total = (unsigned long long)n;
+  KPN_TRY(unstage(c, outs, st));
+  return wd_snapshot(c, st);
 }
 
 extern "C" int kpn_query(kpn_ctx* c, const float* pts, const float* view, int n, float* out5, uint8_t* valid, int mem,
@@ -734,50 +813,16 @@ extern "C" int kpn_query(kpn_ctx* c, const float* pts, const float* view, int n,
   DeviceGuard g(c->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_query");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  int rc = begin_counters(c, st);
-  if (rc != KPN_OK) return rc;
-  if (n == 0) return KPN_OK;
-  const float* dp = pts; const float* dv = view;
-  float* dout = out5; uint8_t* dvalid = valid;
-  if (mem == KPN_MEM_HOST) {
-    size_t fb = (size_t)n * 3 * sizeof(float);
-    KPN_CUDA(c, c->ws_in.reserve(2 * fb));
-    KPN_CUDA(c, cudaMemcpyAsync(c->ws_in.p, pts, fb, cudaMemcpyHostToDevice, st));
-    KPN_CUDA(c, cudaMemcpyAsync(c->ws_in.as<char>() + fb, view, fb, cudaMemcpyHostToDevice, st));
-    dp = c->ws_in.as<float>(); dv = reinterpret_cast<const float*>(c->ws_in.as<char>() + fb);
-    KPN_CUDA(c, c->ws_out.reserve((size_t)n * 5 * sizeof(float) + (size_t)n));
-    dout = c->ws_out.as<float>();
-    dvalid = reinterpret_cast<uint8_t*>(c->ws_out.as<char>() + (size_t)n * 5 * sizeof(float));
-  } else if (!dvalid) {
-    KPN_CUDA(c, c->ws_out.reserve((size_t)n));
-    dvalid = c->ws_out.as<uint8_t>();
-  }
-  const long long chunk = 4ll << 20;
-  const long long nchunks = (n + chunk - 1) / chunk;
-  if (nchunks > MAX_CHUNKS) KPN_FAIL(c, KPN_ERR_ARG, "too many points");
-  for (long long ch = 0; ch < nchunks; ++ch) {
-    long long off = ch * chunk;
-    long long m = (n - off) < chunk ? (n - off) : chunk;
-    SampleSrc src;
-    memset(&src, 0, sizeof(src));
-    src.mode = 1; src.pts = dp + 3 * off; src.view = dv + 3 * off;
-    KPN_CUDA(c, c->ws_list.reserve((size_t)m * sizeof(int)));
-    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + 5 * off, 5, dvalid + off, st));
-    c->launches++;
-    ShadeOut so;
-    memset(&so, 0, sizeof(so));
-    so.out5 = dout + 5 * off;
-    rc = shade_batch(c, src, c->ws_list.as<int>(), c->d_counters + ch, c->d_counters2 + ch, m, 1, so, op ? op->engine : 0, st);
-    if (rc != KPN_OK) return rc;
-  }
-  c->counters_used = (int)nchunks;
-  c->last_total = (unsigned long long)n;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, cudaMemcpyAsync(out5, dout, (size_t)n * 5 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (valid) KPN_CUDA(c, cudaMemcpyAsync(valid, dvalid, (size_t)n, cudaMemcpyDeviceToHost, st));
-  }
-  return wd_snapshot(c, st);
+  KPN_TRY(wd_check(c, st));
+  if (!mem_ok(mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  Staging in(c, true, mem == KPN_MEM_HOST);
+  in.add(pts, (size_t)n * 3 * sizeof(float));
+  in.add(view, (size_t)n * 3 * sizeof(float));
+  KPN_TRY(stage(c, in, st));
+  SampleSrc src;
+  memset(&src, 0, sizeof(src));
+  src.mode = 1; src.pts = in.dev<const float>(0); src.view = in.dev<const float>(1);
+  return query_points(c, src, n, out5, 5, 1, mem, valid, op, st);
 }
 
 extern "C" int kpn_query_grid(kpn_ctx* c, const kpn_grid* g, float* out2, uint8_t* valid, int mem, const kpn_opts* op, void* stream) {
@@ -789,47 +834,15 @@ extern "C" int kpn_query_grid(kpn_ctx* c, const kpn_grid* g, float* out2, uint8_
   for (int a = 0; a < 3; ++a)
     if (!std::isfinite(g->origin[a]) || !std::isfinite(g->spacing[a]) || !(g->spacing[a] > 0.0f))
       KPN_FAIL(c, KPN_ERR_ARG, "grid origin / spacing must be finite, spacing > 0 (axis %d: %g, %g)", a, g->origin[a], g->spacing[a]);
-  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!mem_ok(mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
   if (!c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_scene must precede kpn_query_grid");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
-  int rc = begin_counters(c, st);
-  if (rc != KPN_OK) return rc;
-  const long long n = (long long)g->nx * g->ny * g->nz;
-  float* dout = out2; uint8_t* dvalid = valid;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, c->ws_out.reserve((size_t)n * 2 * sizeof(float) + (size_t)n));
-    dout = c->ws_out.as<float>();
-    dvalid = reinterpret_cast<uint8_t*>(c->ws_out.as<char>() + (size_t)n * 2 * sizeof(float));
-  } else if (!dvalid) {
-    KPN_CUDA(c, c->ws_out.reserve((size_t)n));
-    dvalid = c->ws_out.as<uint8_t>();
-  }
-  const long long chunk = 4ll << 20;   // as kpn_query
-  const long long nchunks = (n + chunk - 1) / chunk;
-  for (long long ch = 0; ch < nchunks; ++ch) {
-    const long long off = ch * chunk;
-    const long long m = (n - off) < chunk ? (n - off) : chunk;
-    SampleSrc src;
-    memset(&src, 0, sizeof(src));
-    src.mode = 2;
-    for (int a = 0; a < 3; ++a) { src.g_org[a] = g->origin[a]; src.g_sp[a] = g->spacing[a]; }
-    src.g_nx = g->nx; src.g_ny = g->ny; src.g_id0 = off;
-    KPN_CUDA(c, c->ws_list.reserve((size_t)m * sizeof(int)));
-    KPN_CUDA(c, launch_compact(c->d_scene, src, m, c->ws_list.as<int>(), c->d_counters + ch, dout + 2 * off, 2, dvalid + off, st));
-    c->launches++;
-    ShadeOut so;
-    memset(&so, 0, sizeof(so));
-    so.out2 = dout + 2 * off;
-    rc = shade_batch(c, src, c->ws_list.as<int>(), c->d_counters + ch, c->d_counters2 + ch, m, 2, so, op ? op->engine : 0, st);
-    if (rc != KPN_OK) return rc;
-  }
-  c->counters_used = (int)nchunks;
-  c->last_total = (unsigned long long)n;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, cudaMemcpyAsync(out2, dout, (size_t)n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (valid) KPN_CUDA(c, cudaMemcpyAsync(valid, dvalid, (size_t)n, cudaMemcpyDeviceToHost, st));
-  }
-  return wd_snapshot(c, st);
+  KPN_TRY(wd_check(c, st));
+  SampleSrc src;
+  memset(&src, 0, sizeof(src));
+  src.mode = 2;
+  for (int a = 0; a < 3; ++a) { src.g_org[a] = g->origin[a]; src.g_sp[a] = g->spacing[a]; }
+  src.g_nx = g->nx; src.g_ny = g->ny;
+  return query_points(c, src, (long long)g->nx * g->ny * g->nz, out2, 2, 2, mem, valid, op, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -840,7 +853,7 @@ extern "C" int kpn_mesh_begin(kpn_ctx* c, const float* field, int nx, int ny, in
   DeviceGuard dg(c->device);
   cudaStream_t st = (cudaStream_t)stream;
   c->mc_field = nullptr;
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  KPN_TRY(wd_check(c, st));
   if (nx < 1 || ny < 1 || nz < 1 || (long long)nx * ny * nz > 0x7fffffffll)
     KPN_FAIL(c, KPN_ERR_ARG, "field %d x %d x %d: every extent >= 1, at most 2^31 - 1 points", nx, ny, nz);
   const int n = nx * ny * nz;
@@ -871,32 +884,25 @@ extern "C" int kpn_mesh_emit(kpn_ctx* c, const float* field, const float origin[
   if (!c || !field || !origin || !spacing) return KPN_ERR_ARG;
   DeviceGuard dg(c->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!mem_ok(mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
   for (int a = 0; a < 3; ++a)
     if (!std::isfinite(origin[a]) || !std::isfinite(spacing[a]) || !(spacing[a] > 0.0f))
       KPN_FAIL(c, KPN_ERR_ARG, "origin / spacing must be finite, spacing > 0 (axis %d: %g, %g)", a, origin[a], spacing[a]);
   if (c->mc_field == nullptr || c->mc_field != field)
     KPN_FAIL(c, KPN_ERR_STATE, "kpn_mesh_begin on the same field must precede kpn_mesh_emit");
-  { int hrc = wd_check(c, st); if (hrc != KPN_OK) return hrc; }
+  KPN_TRY(wd_check(c, st));
   const long long nv = c->mc_counts[0], nf = c->mc_counts[1];
   if ((nv > 0 && !vertices) || (nf > 0 && !faces)) KPN_FAIL(c, KPN_ERR_ARG, "null vertices / faces for a non-empty mesh");
-  float* dv = vertices; float* dn = normals; int* df = faces;
-  const size_t vb = (size_t)nv * 3 * sizeof(float), fb = (size_t)nf * 3 * sizeof(int);
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, c->ws_out.reserve(2 * vb + fb + 16));
-    dv = c->ws_out.as<float>();
-    dn = normals ? reinterpret_cast<float*>(c->ws_out.as<char>() + vb) : nullptr;
-    df = reinterpret_cast<int*>(c->ws_out.as<char>() + 2 * vb);
-  }
+  Staging outs(c, false, mem == KPN_MEM_HOST);
+  outs.add(vertices, (size_t)nv * 3 * sizeof(float));
+  outs.add(normals, (size_t)nv * 3 * sizeof(float));
+  outs.add(faces, (size_t)nf * 3 * sizeof(int));
+  KPN_TRY(stage(c, outs, st));
   KPN_CUDA(c, launch_mc_emit(field, c->mc_dims[0], c->mc_dims[1], c->mc_dims[2], c->mc_level, origin, spacing, c->mc_vofs.as<unsigned int>(),
-                             c->mc_cases.as<uint8_t>(), c->mc_tofs.as<unsigned int>(), dv, dn, df, nf, st));
+                             c->mc_cases.as<uint8_t>(), c->mc_tofs.as<unsigned int>(), outs.dev<float>(0), outs.dev<float>(1),
+                             outs.dev<int>(2), nf, st));
   c->launches += nf > 0 ? 2 : 1;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, cudaMemcpyAsync(vertices, dv, vb, cudaMemcpyDeviceToHost, st));
-    if (normals) KPN_CUDA(c, cudaMemcpyAsync(normals, dn, vb, cudaMemcpyDeviceToHost, st));
-    KPN_CUDA(c, cudaMemcpyAsync(faces, df, fb, cudaMemcpyDeviceToHost, st));
-  }
-  return KPN_OK;
+  return unstage(c, outs, st);
 }
 
 extern "C" int kpn_get_stats(kpn_ctx* c, kpn_stats* stats, void* stream) {
@@ -908,7 +914,7 @@ extern "C" int kpn_get_stats(kpn_ctx* c, kpn_stats* stats, void* stream) {
     KPN_CUDA(c, cudaMemcpyAsync(h.data(), c->d_counters, sizeof(int) * c->counters_used, cudaMemcpyDeviceToHost, st));
     KPN_CUDA(c, cudaMemcpyAsync(h2.data(), c->d_counters2, sizeof(int) * c->counters_used, cudaMemcpyDeviceToHost, st));
   }
-  KPN_CUDA(c, tc_watchdog_read_async(c->h_wd, st));
+  KPN_TRY(wd_snapshot(c, st));
   KPN_CUDA(c, cudaStreamSynchronize(st));
   unsigned long long valid = 0, coloured = 0;
   for (int i = 0; i < c->counters_used; ++i) { valid += (unsigned long long)h[i]; coloured += (unsigned long long)h2[i]; }
@@ -937,9 +943,12 @@ extern "C" int kpn_debug_timing(kpn_ctx* c, int enable, unsigned long long* out1
   if (!c) return KPN_ERR_ARG;
   DeviceGuard g(c->device);
   KPN_CUDA(c, cudaDeviceSynchronize());
-  unsigned int wd[8];
-  KPN_CUDA(c, tc_watchdog_read(wd, enable != 0));
-  if (out16) { for (int i = 0; i < 16; ++i) out16[i] = i < 8 ? wd[i] : 0ull; }
+  unsigned int wd[TC_WD_MODULES * TC_WD_WORDS];
+  KPN_TRY(wd_read(c, wd, nullptr));
+  if (enable) KPN_TRY(wd_clear(c, nullptr));
+  KPN_CUDA(c, cudaDeviceSynchronize());
+  const unsigned int* first = wd[0] != 0u || wd[TC_WD_WORDS] == 0u ? wd : wd + TC_WD_WORDS;   // the first raised module's words
+  if (out16) { for (int i = 0; i < 16; ++i) out16[i] = i < 8 ? first[i] : 0ull; }
   return KPN_OK;
 }
 
@@ -958,15 +967,11 @@ extern "C" int kpn_debug_kmap(int stage, int n_kpt, int n_inputs, int* kmap_out,
   return KPN_OK;
 }
 
-// Debug, instrumented build (-DKPN_STAGE_TIMING) only: cycle stamps of one issuer warp of the geometry kernel (layout in
-// kpn_shade_tc.cu); out receives up to n_words values, *n_tiles the tiles recorded since the last call.
+// Debug, instrumented build (-DKPN_STAGE_TIMING) only: cycle stamps of one issuer warp of the geometry kernel.  This
+// architecture's kernels have no such instrumentation, so every call is refused.
 extern "C" int kpn_debug_stage_times(kpn_ctx* c, unsigned long long* out, int n_words, int* n_tiles) {
   if (!c || !out || !n_tiles) return KPN_ERR_ARG;
-  DeviceGuard g(c->device);
-  cudaError_t e = tc_stage_times(out, n_words, n_tiles);
-  if (e == cudaErrorNotSupported) KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "library was not built with -DKPN_STAGE_TIMING");
-  KPN_CUDA(c, e);
-  return KPN_OK;
+  KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "library was not built with -DKPN_STAGE_TIMING");
 }
 
 extern "C" int kpn_decode_views(kpn_ctx* c, const uint8_t* images, const uint8_t* masks, const double* cams, int n_views, int src_h,
@@ -976,30 +981,20 @@ extern "C" int kpn_decode_views(kpn_ctx* c, const uint8_t* images, const uint8_t
   cudaStream_t st = (cudaStream_t)stream;
   if (n_views < 1 || src_h < 1 || src_w < 1 || factor < 1 || src_h % factor || src_w % factor)
     KPN_FAIL(c, KPN_ERR_ARG, "decode: %d views of %dx%d by 1/%d", n_views, src_h, src_w, factor);
-  if (mem != KPN_MEM_HOST && mem != KPN_MEM_DEVICE) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  if (!mem_ok(mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
   const size_t npx = (size_t)n_views * src_h * src_w, nout = npx / ((size_t)factor * factor);
-  const size_t cam_bytes = (size_t)n_views * 18 * sizeof(double);
-  const uint8_t* d_img = images; const uint8_t* d_msk = masks; const void* d_cam = cams;
-  float* d_out = out_img; uint8_t* d_om = out_mask;
-  if (mem == KPN_MEM_HOST) {
-    // staging layout: cams | images | masks | out_img | out_mask
-    const size_t off_img = (cam_bytes + 255) / 256 * 256, off_msk = off_img + (npx * 3 + 255) / 256 * 256;
-    const size_t off_out = off_msk + (npx + 255) / 256 * 256, off_om = off_out + nout * 3 * sizeof(float);
-    KPN_CUDA(c, c->ws_in.reserve(off_om + nout));
-    char* b = c->ws_in.as<char>();
-    KPN_CUDA(c, cudaMemcpyAsync(b, cams, cam_bytes, cudaMemcpyHostToDevice, st));
-    KPN_CUDA(c, cudaMemcpyAsync(b + off_img, images, npx * 3, cudaMemcpyHostToDevice, st));
-    if (masks) KPN_CUDA(c, cudaMemcpyAsync(b + off_msk, masks, npx, cudaMemcpyHostToDevice, st));
-    d_cam = b; d_img = reinterpret_cast<uint8_t*>(b + off_img); d_msk = masks ? reinterpret_cast<uint8_t*>(b + off_msk) : nullptr;
-    d_out = reinterpret_cast<float*>(b + off_out); d_om = out_mask ? reinterpret_cast<uint8_t*>(b + off_om) : nullptr;
-  }
-  KPN_CUDA(c, launch_decode_views(d_img, d_msk, d_cam, n_views, src_h, src_w, factor, d_out, d_om, st));
+  Staging in(c, true, mem == KPN_MEM_HOST), outs(c, false, mem == KPN_MEM_HOST);
+  in.add(cams, (size_t)n_views * 18 * sizeof(double));
+  in.add(images, npx * 3);
+  in.add(masks, npx);
+  outs.add(out_img, nout * 3 * sizeof(float));
+  outs.add(out_mask, nout);
+  KPN_TRY(stage(c, in, st));
+  KPN_TRY(stage(c, outs, st));
+  KPN_CUDA(c, launch_decode_views(in.dev<const uint8_t>(1), in.dev<const uint8_t>(2), in.dev<const void>(0), n_views, src_h, src_w,
+                                  factor, outs.dev<float>(0), outs.dev<uint8_t>(1), st));
   c->launches++;
-  if (mem == KPN_MEM_HOST) {
-    KPN_CUDA(c, cudaMemcpyAsync(out_img, d_out, nout * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (out_mask) KPN_CUDA(c, cudaMemcpyAsync(out_mask, d_om, nout, cudaMemcpyDeviceToHost, st));
-  }
-  return KPN_OK;
+  return unstage(c, outs, st);
 }
 
 extern "C" int kpn_set_profiling(kpn_ctx* c, int enable) {

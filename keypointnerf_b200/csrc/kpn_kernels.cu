@@ -1005,9 +1005,7 @@ cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n
   return cudaGetLastError();
 }
 template <int NV, int TS>
-static cudaError_t launch_shade_simt_tile(const DevScene* sc, const DevWeightsF32* W, const SampleSrc& src, const int* list,
-                                          const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
-                                          cudaStream_t st) {
+static cudaError_t launch_shade_simt_tile(const ShadeBatch& b) {
   constexpr size_t smem = SHADE_SMEM_BYTES<NV, TS>;
   static std::atomic<bool> attr_set[64];   // function attributes are per device (setting them twice is harmless)
   int dev = 0;
@@ -1017,16 +1015,16 @@ static cudaError_t launch_shade_simt_tile(const DevScene* sc, const DevWeightsF3
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
-  int grid = grid_for(n_max, TS, num_sms);
-  shade_simt_kernel<NV, TS><<<grid, 4 * TS, smem, st>>>(sc, W, src, list, counter, query_mode, so);
-  return cudaGetLastError();
+  int grid = grid_for(b.n_max, TS, b.num_sms);
+  shade_simt_kernel<NV, TS><<<grid, 4 * TS, smem, b.st>>>(b.sc, b.wf32, b.src, b.list, b.counter, b.query_mode, b.so);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  *b.launches += 1;
+  return b.after_geo ? cudaEventRecord(b.after_geo, b.st) : cudaSuccess;
 }
-cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,
-                              const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
-                              cudaStream_t st) {
-  if (n_views < 1 || n_views > MAXV) return cudaErrorInvalidValue;
-  return n_views <= 3 ? launch_shade_simt_tile<3, 64>(sc, W, src, list, counter, n_max, query_mode, so, num_sms, st)
-                      : launch_shade_simt_tile<4, 56>(sc, W, src, list, counter, n_max, query_mode, so, num_sms, st);
+cudaError_t launch_shade_simt(const ShadeBatch& b) {
+  if (b.n_views < 1 || b.n_views > MAXV) return cudaErrorInvalidValue;
+  return b.n_views <= 3 ? launch_shade_simt_tile<3, 64>(b) : launch_shade_simt_tile<4, 56>(b);
 }
 cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb, const int* start0, const int* cnt0,
                              const int* start1, const int* cnt1, const float* zbuf, const float* ray_nf, int r0, int nr, int S,

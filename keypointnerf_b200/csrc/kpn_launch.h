@@ -18,38 +18,51 @@ cudaError_t launch_front(const DevScene* sc, const DevTarget* tg, int nr, int S,
                          int* ray_cnt, const ErtSegment& ert, cudaStream_t st);
 cudaError_t launch_compact(const DevScene* sc, const SampleSrc& src, long long n, int* list, int* counter, float* out, int out_w,
                            uint8_t* valid_out, cudaStream_t st);
-cudaError_t launch_shade_simt(const DevScene* sc, int n_views, const DevWeightsF32* W, const SampleSrc& src, const int* list,
-                              const int* counter, long long n_max, int query_mode, const ShadeOut& so, int num_sms,
-                              cudaStream_t st);
 cudaError_t launch_composite(const int* list, const float2* ao, const float* rgb, const int* start0, const int* cnt0,
                              const int* start1, const int* cnt1, const float* zbuf, const float* ray_nf, int r0, int nr, int S,
                              long long plane, float* color, float* depth, float* alpha, float* sdf, float* ray_alpha, float* cw,
                              cudaStream_t st);
 cudaError_t launch_resample(const int* list, const float* cw, const int* start0, const int* cnt0, const int* start1, const int* cnt1,
                             const float* ray_nf, int nr, int Sc, int Sf, float* zout, float* contrib_out, cudaStream_t st);
-// Tensor-core engine: geometry front (L0-L3 + pooling) and density tail kernels, then the colour kernel on the samples with
-// density > 0 (query_mode 2: no colour kernel).  n_views: 3 or 4 (the scene's view count, tc_supported); wblob: full fp16 W_hi tiles of every stage; wlo: W_lo
-// tiles of stages 4, 5 (tc_weight_lo_bytes); lat_scratch: n_max x 48 bytes, pool_scratch: tc_pool_bytes(n_max), list2:
-// n_max x int2, count2: device int (zeroed by the caller).  *launches is incremented by the number of kernels enqueued.
-cudaError_t launch_shade_tc(const DevScene* sc, int n_views, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term,
-                            int n_kpt, const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                            const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
-                            cudaEvent_t after_geo, int* launches, cudaStream_t st);
-// the 4-view instantiation (kpn_shade_tc_v4.cu); lo_mask as launch_shade_tc derives it from two_term
-cudaError_t launch_shade_tc_v4(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask, int n_kpt,
-                               const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                               const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
-                               cudaEvent_t after_geo, int* launches, cudaStream_t st);
+// One shading batch: the samples of list[0 .. *counter) (device-side count, at most n_max) of src, shaded with the scene sc
+// (n_views views, n_kpt keypoints); `so` says where the results go.  Built once per batch (kpn_api.cu) and passed to the engine's
+// launcher, which records after_geo (if not null) once the geometry is shaded and adds the kernels it enqueues to *launches.
+struct ShadeBatch {
+  const DevScene* sc;
+  int n_views, n_kpt;
+  SampleSrc src;
+  const int* list;
+  const int* counter;
+  long long n_max;
+  int query_mode;
+  ShadeOut so;
+  int num_sms;
+  cudaStream_t st;
+  const DevWeightsF32* wf32;   // fp32 engine
+  // tensor-core engine: geometry front (L0-L3 + pooling) and density tail kernels, then the colour kernel on the samples with
+  // density > 0 (query_mode 2: no colour kernel).  n_views: 3 or 4 (tc_supported); wblob: full fp16 W_hi tiles of every stage;
+  // wlo: W_lo tiles of stages 4, 5 (tc_weight_lo_bytes); lo_mask: the W_lo and A_lo passes of the density tail (stages 4, 5:
+  // bits 4, 5 and 6, 7); lat: n_max x 48 bytes, pool: tc_pool_bytes(n_max), list2: n_max entries, count2: device int (zeroed by
+  // the caller).
+  const TcConsts* tcc;
+  const uint8_t *wblob, *wlo;
+  int lo_mask;
+  uint4* lat;
+  float* pool;
+  int2* list2;
+  int* count2;
+  cudaEvent_t after_geo;
+  unsigned long long* launches;
+};
+cudaError_t launch_shade_simt(const ShadeBatch& b);
+cudaError_t launch_shade_tc(const ShadeBatch& b);
+cudaError_t launch_shade_tc_v4(const ShadeBatch& b);   // the 4-view instantiation (kpn_shade_tc_v4.cu)
 size_t tc_pool_bytes(long long n_max);
 // Device watchdog words of the tensor-core kernels: TC_WD_WORDS per module, one module per view-count translation unit.
 constexpr int TC_WD_WORDS = 8;
 constexpr int TC_WD_MODULES = 2;
-cudaError_t tc_watchdog_read(unsigned int out[8], bool reset);   // the first module whose flag is raised (else the first module)
-// stream-ordered copy of every module's words into pinned host memory (TC_WD_MODULES x TC_WD_WORDS)
-cudaError_t tc_watchdog_read_async(unsigned int* pinned_out, cudaStream_t st);
-cudaError_t tc_watchdog_clear_async(cudaStream_t st);
+cudaError_t tc_watchdog_words(void* w[TC_WD_MODULES]);   // device address of every module's words
 cudaError_t tc_watchdog_addr_v4(void** p);   // device address of the 4-view module's words
-cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles);   // not supported: cudaErrorNotSupported
 size_t tc_weight_blob_bytes(int n_kpt);
 size_t tc_weight_lo_bytes(int n_kpt);
 bool tc_supported(int n_views, int n_kpt, int sp_level);

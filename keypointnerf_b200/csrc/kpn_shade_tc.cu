@@ -231,58 +231,18 @@ cudaError_t launch_colour_list(const int* list, const int* counter, const float2
   return cudaGetLastError();
 }
 
-cudaError_t launch_shade_tc(const DevScene* sc, int n_views, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int two_term,
-                            int n_kpt, const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                            const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
-                            cudaEvent_t after_geo, int* launches, cudaStream_t st) {
-  // W_lo and A_lo passes of the density tail (stages 4, 5: bits 4, 5 and 6, 7); single-term weights keep the A_lo passes
-  const int lo_mask = two_term ? 0xF0 : 0xC0;
-  if (n_views == 3)
-    return launch_tc_views<3>(sc, C, wblob, wlo, lo_mask, n_kpt, src, list, counter, n_max, query_mode, so, lat_scratch, pool_scratch,
-                              list2, count2, num_sms, after_geo, launches, st);
-  if (n_views == 4)
-    return launch_shade_tc_v4(sc, C, wblob, wlo, lo_mask, n_kpt, src, list, counter, n_max, query_mode, so, lat_scratch, pool_scratch,
-                              list2, count2, num_sms, after_geo, launches, st);
+cudaError_t launch_shade_tc(const ShadeBatch& b) {
+  if (b.n_views == 3) return launch_tc_views<3>(b);
+  if (b.n_views == 4) return launch_shade_tc_v4(b);
   return cudaErrorInvalidValue;
 }
 
 // Watchdog state of the tensor-core kernels.  Every translation unit has its own copy of the words (kpn_tc.cuh): the 3-view
-// module's (with the shared tail kernel) and the 4-view module's; out[0] != 0 -> some barrier wait gave up at block out[1],
-// thread out[2], tag out[3].
+// module's (with the shared tail kernel) and the 4-view module's.
 static_assert(TC_WD_MODULES == 2, "the 3-view and the 4-view module");
-static cudaError_t wd_words(void* w[TC_WD_MODULES]) {
+cudaError_t tc_watchdog_words(void* w[TC_WD_MODULES]) {
   cudaError_t e = cudaGetSymbolAddress(&w[0], tc::kpn_wd);
   return e != cudaSuccess ? e : tc_watchdog_addr_v4(&w[1]);
-}
-cudaError_t tc_watchdog_read(unsigned int out[8], bool reset) {
-  void* w[TC_WD_MODULES];
-  unsigned int both[TC_WD_MODULES * TC_WD_WORDS];
-  cudaError_t e = wd_words(w);
-  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m) e = cudaMemcpy(both + TC_WD_WORDS * m, w[m], TC_WD_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return e;
-  const unsigned int* first = both[0] != 0u || both[TC_WD_WORDS] == 0u ? both : both + TC_WD_WORDS;
-  for (int i = 0; i < 8; ++i) out[i] = first[i];
-  for (int m = 0; m < TC_WD_MODULES && reset && e == cudaSuccess; ++m) e = cudaMemset(w[m], 0, TC_WD_WORDS * sizeof(unsigned int));
-  return e;
-}
-
-cudaError_t tc_watchdog_read_async(unsigned int* pinned_out, cudaStream_t st) {
-  void* w[TC_WD_MODULES];
-  cudaError_t e = wd_words(w);
-  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m)
-    e = cudaMemcpyAsync(pinned_out + TC_WD_WORDS * m, w[m], TC_WD_WORDS * sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
-  return e;
-}
-cudaError_t tc_watchdog_clear_async(cudaStream_t st) {
-  void* w[TC_WD_MODULES];
-  cudaError_t e = wd_words(w);
-  for (int m = 0; m < TC_WD_MODULES && e == cudaSuccess; ++m) e = cudaMemsetAsync(w[m], 0, TC_WD_WORDS * sizeof(unsigned int), st);
-  return e;
-}
-// stage-timing instrumentation is not built for this architecture's kernels
-cudaError_t tc_stage_times(unsigned long long* out, int n_words, int* n_tiles) {
-  (void)out; (void)n_words; (void)n_tiles;
-  return cudaErrorNotSupported;
 }
 
 }  // namespace kpn

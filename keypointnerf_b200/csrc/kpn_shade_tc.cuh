@@ -878,10 +878,7 @@ inline int tc_grid(long long tiles, int per_cta, int num_sms) {
 }
 
 template <int NV, int NP>
-cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask,
-                           const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                           const ShadeOut& so, uint4* lat, float* pool, int2* list2, int* count2, int num_sms, cudaEvent_t after_geo,
-                           int* launches, cudaStream_t st) {
+cudaError_t launch_tc_impl(const ShadeBatch& b) {
   constexpr int NK = 2 * NP, FWG = front_wgs(NK, NV), FSPT = fspt(NV), SPT = spt(NV);
   constexpr TcPlan plan = make_tc_plan(NK);
   const size_t smem_front = front_smem_bytes(NK, FWG);
@@ -896,34 +893,38 @@ cudaError_t launch_tc_impl(const DevScene* sc, int nk, const TcConsts& C, const 
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
-  const uint8_t* wtail = wblob + plan.st[4].off;
-  const uint8_t* wcol = wblob + plan.st[GEO_NSTAGE].off;
+  const uint8_t* wtail = b.wblob + plan.st[4].off;
+  const uint8_t* wcol = b.wblob + plan.st[GEO_NSTAGE].off;
   cudaError_t e = cudaSuccess;
   // the device-side count is not known here: every slice of [0, n_max) is launched, slices past the count exit at once
-  const long long nslices = n_max > POOL_SLICE ? (n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
+  const long long nslices = b.n_max > POOL_SLICE ? (b.n_max + POOL_SLICE - 1) / POOL_SLICE : 1;
   for (long long s = 0; s < nslices; ++s) {
-    const long long base = s * POOL_SLICE, len = n_max - base < POOL_SLICE ? n_max - base : POOL_SLICE;
-    auto front = src.mode == 2 ? geo_front_kernel<NV, NP, true> : geo_front_kernel<NV, NP, false>;
-    front<<<tc_grid((len + FSPT - 1) / FSPT, FWG, num_sms), FWG * 128, smem_front, st>>>(sc, nk, wblob, src, list, counter, base, len,
-                                                                                         pool);
-    e = launch_geo_tail(C, wtail, wlo, lo_mask, list, counter, base, len, pool, query_mode, so, lat, num_sms, st);
+    const long long base = s * POOL_SLICE, len = b.n_max - base < POOL_SLICE ? b.n_max - base : POOL_SLICE;
+    auto front = b.src.mode == 2 ? geo_front_kernel<NV, NP, true> : geo_front_kernel<NV, NP, false>;
+    front<<<tc_grid((len + FSPT - 1) / FSPT, FWG, b.num_sms), FWG * 128, smem_front, b.st>>>(b.sc, b.n_kpt, b.wblob, b.src, b.list,
+                                                                                             b.counter, base, len, b.pool);
+    e = launch_geo_tail(*b.tcc, wtail, b.wlo, b.lo_mask, b.list, b.counter, base, len, b.pool, b.query_mode, b.so, b.lat, b.num_sms,
+                        b.st);
     if (e != cudaSuccess) return e;
-    *launches += 2;
+    *b.launches += 2;
   }
-  if (after_geo) { e = cudaEventRecord(after_geo, st); if (e != cudaSuccess) return e; }
-  if (query_mode == 2) return cudaSuccess;   // geometry only: no colour work list, no colour kernel
-  const int grid = tc_grid((n_max + SPT - 1) / SPT, CWG, num_sms);
-  if (query_mode) {   // every valid sample gets a colour: the first list is the colour work list
-    shade_color_kernel<NV><<<grid, CWG * 128, COL_SMEM, st>>>(sc, C, wcol, src, nullptr, list, counter, lat, query_mode, so);
+  if (b.after_geo) { e = cudaEventRecord(b.after_geo, b.st); if (e != cudaSuccess) return e; }
+  if (b.query_mode == 2) return cudaSuccess;   // geometry only: no colour work list, no colour kernel
+  const int grid = tc_grid((b.n_max + SPT - 1) / SPT, CWG, b.num_sms);
+  if (b.query_mode) {   // every valid sample gets a colour: the first list is the colour work list
+    shade_color_kernel<NV><<<grid, CWG * 128, COL_SMEM, b.st>>>(b.sc, *b.tcc, wcol, b.src, nullptr, b.list, b.counter, b.lat,
+                                                                b.query_mode, b.so);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    *launches += 1;
-    return cudaMemcpyAsync(count2, counter, sizeof(int), cudaMemcpyDeviceToDevice, st);   // statistics: every valid sample was coloured
+    *b.launches += 1;
+    // statistics: every valid sample was coloured
+    return cudaMemcpyAsync(b.count2, b.counter, sizeof(int), cudaMemcpyDeviceToDevice, b.st);
   }
-  e = launch_colour_list(list, counter, so.ao, so.list_base, list2, count2, n_max, num_sms, st);
+  e = launch_colour_list(b.list, b.counter, b.so.ao, b.so.list_base, b.list2, b.count2, b.n_max, b.num_sms, b.st);
   if (e != cudaSuccess) return e;
-  shade_color_kernel<NV><<<grid, CWG * 128, COL_SMEM, st>>>(sc, C, wcol, src, list2, nullptr, count2, lat, query_mode, so);
-  *launches += 2;
+  shade_color_kernel<NV><<<grid, CWG * 128, COL_SMEM, b.st>>>(b.sc, *b.tcc, wcol, b.src, b.list2, nullptr, b.count2, b.lat,
+                                                              b.query_mode, b.so);
+  *b.launches += 2;
   return cudaGetLastError();
 }
 
@@ -935,15 +936,11 @@ constexpr std::array<LaunchTc, sizeof...(I)> launch_table(std::integer_sequence<
 
 // The tensor-core engine for NV source views: launch_tc_impl<NV, NP> for NP = 1 .. KPN_MAX_KPT / 2 keypoint pairs.
 template <int NV>
-cudaError_t launch_tc_views(const DevScene* sc, const TcConsts& C, const uint8_t* wblob, const uint8_t* wlo, int lo_mask, int n_kpt,
-                            const SampleSrc& src, const int* list, const int* counter, long long n_max, int query_mode,
-                            const ShadeOut& so, void* lat_scratch, void* pool_scratch, void* list2, int* count2, int num_sms,
-                            cudaEvent_t after_geo, int* launches, cudaStream_t st) {
+cudaError_t launch_tc_views(const ShadeBatch& b) {
   static constexpr std::array<LaunchTc, KPN_MAX_KPT / 2> table =
       launch_table<NV>(std::make_integer_sequence<int, KPN_MAX_KPT / 2>{});
-  if (n_kpt < 1 || n_kpt > KPN_MAX_KPT) return cudaErrorInvalidValue;
-  return table[tc_npair(n_kpt) - 1](sc, n_kpt, C, wblob, wlo, lo_mask, src, list, counter, n_max, query_mode, so,
-                                    (uint4*)lat_scratch, (float*)pool_scratch, (int2*)list2, count2, num_sms, after_geo, launches, st);
+  if (b.n_kpt < 1 || b.n_kpt > KPN_MAX_KPT) return cudaErrorInvalidValue;
+  return table[tc_npair(b.n_kpt) - 1](b);
 }
 
 }  // namespace

@@ -44,7 +44,7 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
 }
 // Watchdog.  A barrier wait that has not completed after ~2^20 suspended polls is a protocol bug; instead of hanging the GPU
 // the waiter records where it gave up, raises this module's abort flag (every other wait then gives up within 256 polls) and
-// returns, so that the kernel terminates (with garbage results) and the host can report the location (tc_watchdog_read).
+// returns, so that the kernel terminates (with garbage results) and the host can report the location (kpn_check_health).
 static __device__ unsigned int kpn_wd[8];   // [0] flag, [1] block, [2] thread, [3] tag, [4] parity
 __device__ __forceinline__ bool wd_give_up(uint32_t spins, uint32_t limit, uint32_t tag, uint32_t parity) {
   const bool aborted = *reinterpret_cast<volatile unsigned int*>(&kpn_wd[0]) != 0u;
