@@ -293,7 +293,8 @@ int kpn_set_profiling(kpn_ctx* ctx, int enable);
 
 /* Unit test hook for the tensor-core primitive (tests/test_gpu_umma.py): D(128,N) fp32 = A(128,K) fp16 * B(N,K)^T fp16
  * on one warpgroup through wgmma.mma_async (two 64-row MMAs), operands in the shared-memory layouts the kernels use.
- * Device pointers.  N in {16, 32, 48, 64, 96, 112, 128, 144, 192}, K % 16 == 0, K <= 256; variant must be 0. */
+ * Device pointers.  N in {16, 32, 48, 64, 96, 112, 128, 144, 192}, K % 16 == 0, K <= 256; variant 0: A from shared memory,
+ * variant 1: A from registers, (N, K) = (128, 144) or (64, 128) only. */
 int kpn_selftest_umma(int N, int K, const void* A, const void* B, float* D, int variant, void* stream);
 /* Same on a 2-CTA cluster: D(256,N) = A(256,K) * B(N,K)^T, each CTA holding half of B's rows and fetching the other half from
  * its peer's shared memory (distributed shared memory) before its wgmma; N in {32, 64, 96, 128, 192}.  The activation tile is

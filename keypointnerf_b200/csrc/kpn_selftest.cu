@@ -53,6 +53,55 @@ static int run_selftest(int K, const void* A, const void* B, float* D, cudaStrea
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
+// The same tile with the A operand in registers (WgmmaRA), as the geometry front kernel feeds layers 1-3: each thread loads its
+// warp's fragments of all KCH k-blocks from global memory and the warpgroup issues the KCH MMAs of a 64-row half as one group.
+template <int N, int KCH>
+__global__ void __launch_bounds__(128, 1)
+wgmma_ra_selftest_kernel(const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  constexpr int K = 16 * KCH;
+  const int t = threadIdx.x, w = t >> 5, l = t & 31;
+  for (int idx = t; idx < N * K; idx += 128) {
+    const int n = idx / K, k = idx % K;
+    *reinterpret_cast<__half*>(smem + tc::core_offset_bytes(n, k, N)) = B[idx];
+  }
+  tc::fence_proxy_async_smem();
+  __syncthreads();
+  const uint32_t b_lbo = (uint32_t)(N / 8) * 128u;
+  for (int half = 0; half < 2; ++half) {
+    uint32_t a[4 * KCH];
+#pragma unroll
+    for (int j = 0; j < KCH; ++j)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = 64 * half + 16 * w + (l >> 2) + 8 * (i & 1), k = 16 * j + 8 * (i >> 1) + 2 * (l & 3);
+        const __half2 h = __halves2half2(A[(size_t)r * K + k], A[(size_t)r * K + k + 1]);
+        a[4 * j + i] = *reinterpret_cast<const uint32_t*>(&h);
+      }
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.0f;
+    tc::wg_fence();
+    tc::wg_mma_ra<N, KCH>(d, a, tc::smem_u32(smem), b_lbo, 0u);
+    tc::wg_commit();
+    tc::wg_wait0();
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      const int r = 64 * half + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      D[(size_t)r * N + c] = d[i];
+    }
+  }
+}
+
+template <int N, int KCH>
+static int run_ra_selftest(const void* A, const void* B, float* D, cudaStream_t st) {
+  const size_t smem = (size_t)N * KCH * 16 * 2;
+  if (cudaFuncSetAttribute(wgmma_ra_selftest_kernel<N, KCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return -2;
+  wgmma_ra_selftest_kernel<N, KCH><<<1, 128, smem, st>>>((const __half*)A, (const __half*)B, D);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
 
 // CTA-pair form on a 2-CTA cluster: D[256][N] = A[256][K] * B[N][K]^T.  CTA r holds rows 128r .. 128r+127 of A and keeps rows
 // r*N/2 .. (r+1)*N/2-1 of B; the other half of B comes from the peer CTA's shared memory (distributed shared memory), then each
@@ -146,10 +195,16 @@ static int run_pair_selftest(int K, const void* A, const void* B, float* D, int 
 }  // namespace kpn
 
 // A (128,K) fp16, B (N,K) fp16, D (128,N) fp32: device pointers.  N in {16, 32, 48, 64, 96, 112, 128, 144, 192} (the widths
-// with a wgmma instantiation), K % 16 == 0, K <= 256.  variant 0 is the only operand arrangement (the one the kernels use).
+// with a wgmma instantiation), K % 16 == 0, K <= 256.  variant 0: A from the activation tile in shared memory; variant 1: A from
+// registers, for the shapes of the front kernel's layers 1-3, (N, K) = (128, 144) and (64, 128).
 extern "C" int kpn_selftest_umma(int N, int K, const void* A, const void* B, float* D, int variant, void* stream) {
-  if (K % 16 || K < 16 || K > 256 || variant != 0) return -1;
+  if (K % 16 || K < 16 || K > 256 || variant < 0 || variant > 1) return -1;
   cudaStream_t st = (cudaStream_t)stream;
+  if (variant == 1) {
+    if (N == 128 && K == 144) return kpn::run_ra_selftest<128, 9>(A, B, D, st);
+    if (N == 64 && K == 128) return kpn::run_ra_selftest<64, 8>(A, B, D, st);
+    return -1;
+  }
   switch (N) {
     case 16: return kpn::run_selftest<16>(K, A, B, D, st);
     case 32: return kpn::run_selftest<32>(K, A, B, D, st);

@@ -279,9 +279,9 @@ __device__ __forceinline__ void pool_views(const float* w, const float4* x, floa
 }
 
 // =====================================================================================================================
-// geometry front: stages L0-L3 + view pooling.  Warpgroup tile = 64 rows: row warps 0/1 hold rows 0-31 / 32-63 with
-// column half h = 0, row warps 2/3 the same rows with h = 1 (the two threads of a row split the layer-0 input build and the
-// pooling columns, as tc_kmap's runs are laid out).  2 * spw(NV) samples per tile: 20 with 3 views, 16 with 4.
+// geometry front: stages L0-L3 + view pooling.  Warpgroup tile = 64 rows: row warps 0/1 hold rows 0-31 with column half
+// h = 0 / 1, row warps 2/3 rows 32-63 (the two threads of a row split the layer-0 input build, as tc_kmap's runs are laid
+// out), so that each warp's wgmma fragment rows are rows of its own lanes.  2 * spw(NV) samples per tile: 20 with 3 views, 16 with 4.
 // =====================================================================================================================
 constexpr int GWG = 2;                        // warpgroups per CTA of the tail kernel (the front kernel's: front_wgs)
 __host__ __device__ constexpr int fspt(int nv) { return 2 * spw(nv); }   // samples per front tile
@@ -367,7 +367,7 @@ __device__ __forceinline__ void encode_pair(const SceneS<NV>& S, int v, int j, i
 }
 
 // feat64 channels of the layer-0 input (reference src/utils.py:74-89), loaded a whole 128-byte line per row at a time.  The row
-// warps wq and wq + 2 hold the same 32 rows (lane = row); warp h gathers all 64 channels of its lanes 16h .. 16h + 15, four rows
+// warps 2 rh and 2 rh + 1 hold the same 32 rows (lane = row); warp h gathers all 64 channels of its lanes 16h .. 16h + 15, four rows
 // per step: lanes 8g .. 8g + 7 take row 16h + 4k + g of step k, and lane l8 = lane & 7 loads float4 groups l8 and l8 + 8 of that
 // row's four taps (each load instruction reads four whole lines, one per row; with a lane per row it read ~30 lines of 16 bytes
 // each).  The row's tap offsets and weights come from its lane by shuffles.  Each channel is blended with gather_f32's
@@ -418,19 +418,137 @@ __device__ __forceinline__ void gather_feat8(const SceneS<NV>& S, int v, const P
   w[1] = tc::pack_h2(g8[2], g8[3]);
 }
 
+// Layer-0 input of one tile, this thread's part (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather),
+// column order tc_kmap: thread h of row `row` writes the keypoint encodings of its run (and thread 1 the bias column and K
+// padding); the feat64 words of both runs come from gather_feat64.
+template <int NV, int NP>
+__device__ __forceinline__ void front_l0_encode(const SceneS<NV>& scs, int v, int nk, const float p[3], uint8_t* A, int row, int h) {
+  constexpr int NK = 2 * NP, PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
+  float c[3];
+  const float* E = scs.E[v];
+  c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
+  c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
+  c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
+  constexpr int C1 = 7 * PA + FA / 2;             // thread 0's run: words [0, C1); thread 1's: [C1, K0P / 2)
+  static_assert(C1 % 4 == 0 && C1 > 0, "both runs start on a 16-byte chunk");
+  if (h == 0) {
+    if constexpr (PA > 0) {
+      uint32_t a[7 * PA];
+#pragma unroll
+      for (int j = 0; j < PA; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * j);
+      a_put_span<0, 7 * PA>(A, row, a);
+    }
+  } else {
+    constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
+    constexpr int N1 = tc_k0p(NK) / 2 - C1;
+    static_assert(NE + NF + 1 <= N1, "the bias column is in thread 1's run");
+    uint32_t a[NE > 0 ? NE : 1];
+#pragma unroll
+    for (int j = PA; j < NP; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * (j - PA));
+    if constexpr (NE > 0) a_put_span<C1, NE>(A, row, a);
+    uint32_t b[N1 - NE - NF];
+    b[0] = H2_ONE;
+#pragma unroll
+    for (int i = 1; i < N1 - NE - NF; ++i) b[i] = 0u;
+    a_put_span<C1 + NE + NF, N1 - NE - NF>(A, row, b);
+  }
+}
+
+// L3 rows (d3: the m64n64 accumulator fragment) and the rows' view weights to shared memory over the warpgroup's activation tile,
+// then the view pooling: weighted mean || variance over the NV rows of a sample (src/utils.py:722-748), one (sample, 4 columns)
+// item per thread at a time.  The caller has retired every MMA that reads the tile; on return the tile is free again.
+template <int NV>
+__device__ __forceinline__ void front_pool(const float* d3, float pw, float* D3, int wq, int lane, int row, int h, long long base,
+                                           long long end, int tile, float* __restrict__ pool, int bar_id) {
+  constexpr int SPW = spw(NV), FSPT = fspt(NV);
+#pragma unroll
+  for (int m = 0; m < 16; ++m) {
+    const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 8 * (m >> 1) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(D3 + r * D3S + c) = make_float2(d3[2 * m], d3[2 * m + 1]);
+  }
+  if (h == 0) D3[64 * D3S + row] = pw;
+  tc::named_sync(bar_id, 128);
+  for (int it = 32 * wq + lane; it < FSPT * 16; it += 128) {
+    const int s = it >> 4, c = 4 * (it & 15);
+    const int r0 = (s / SPW) * 32 + NV * (s % SPW);   // row of the sample's view 0
+    float4 x[NV];
+    float w[NV];
+#pragma unroll
+    for (int u = 0; u < NV; ++u) {
+      x[u] = *reinterpret_cast<const float4*>(D3 + (r0 + u) * D3S + c);
+      w[u] = D3[64 * D3S + r0 + u];
+    }
+    float4 mn, vr;
+    pool_views<NV>(w, x, mn, vr);
+    const long long sj = base + (long long)tile * FSPT + s;
+    if (sj < end) {
+      float* out = pool + (sj - base) * POOL_W + c;
+      *reinterpret_cast<float4*>(out) = mn;
+      *reinterpret_cast<float4*>(out + 64) = vr;
+    }
+  }
+  tc::named_sync(bar_id, 128);   // the L3 rows are read: the next tile's input may overwrite them
+}
+
+// Softplus epilogue of a 128-wide stage into the next layer's A fragments (pipelined form): a[m] is the word front_epi_sp stores at
+// row 16 wq + (lane >> 2) + 8 (m & 1), word column 4 (m >> 1) + (lane & 3), so a[4j .. 4j + 3] is k-block j (WgmmaRA).
+__device__ __forceinline__ void front_sp_frag(const float* d, uint32_t* a) {
+#pragma unroll
+  for (int m = 0; m < 32; ++m) a[m] = sp_pair(__float_as_uint(d[2 * m]), __float_as_uint(d[2 * m + 1]));
+}
+
+// One register-A stage of the pipelined form: front_ra_issue starts it, front_ra_wait retires it.  The fences keep the fragment's
+// definitions before the chain and the accumulators' reads after the wait (ptxas keeps the fragment's registers until the wait).
+template <int N, int KCH>
+__device__ __forceinline__ void front_ra_issue(float* d, uint32_t* a, uint32_t b) {
+  tc::fence_regs<4 * KCH>(a);
+  tc::fence_regs<N / 2>(d);
+  tc::wg_fence();
+  tc::wg_mma_ra<N, KCH>(d, a, b, (uint32_t)(N / 8) * 128u, 0u);
+  tc::wg_commit();
+}
+template <int N>
+__device__ __forceinline__ void front_ra_wait(float* d) {
+  tc::wg_wait0();
+  tc::fence_regs<N / 2>(d);
+}
+
+// feat8 words 64..67 of the layer-2 input as the first two registers of k-block 8's A fragment (rows 16 wq + (lane >> 2) and + 8,
+// word 64 + (lane & 3)).  A warp's 16 fragment rows are the rows of its lanes 16 (wq & 1) .. + 15 (the row threads' mapping in
+// geo_front_kernel): lane l gathers channels [4 (l >> 4), + 4) of fragment row l & 15 from that row thread's projection (the
+// same taps and blend as gather_feat8 in the row thread), and the fragment lanes take their words by shuffles.
+template <int NV>
+__device__ __forceinline__ void gather_feat8_frag(const SceneS<NV>& S, const Proj& q, int wq, int lane, uint32_t f8[2]) {
+  const int rl = 16 * (wq & 1) + (lane & 15);
+  Proj qr;
+  qr.u = __shfl_sync(FULL, q.u, rl);
+  qr.v = __shfl_sync(FULL, q.v, rl);
+  qr.zn = 0.0f;
+  uint32_t w[2];
+  gather_feat8(S, rl % NV, qr, lane >> 4, w);
+  const int t = lane & 3, s0 = (lane >> 2) + 16 * (t >> 1);
+  const uint32_t x0 = __shfl_sync(FULL, w[0], s0), x1 = __shfl_sync(FULL, w[1], s0);
+  const uint32_t y0 = __shfl_sync(FULL, w[0], s0 + 8), y1 = __shfl_sync(FULL, w[1], s0 + 8);
+  f8[0] = (t & 1) ? x1 : x0;
+  f8[1] = (t & 1) ? y1 : y0;
+}
+
 // Latency options of a front instantiation's tile chain:
 //   FO_F8_EARLY     the feat8 words are gathered at the start of the tile, beside the feat64 gather, and held until the layer-2
 //                   input is built (otherwise they are gathered there, and the chain waits on a global load between L1 and L2);
 //   FO_NEXT_ID      the next tile's work-list entry is loaded at the start of the tile, so the tile after it starts on one global
 //                   load (the sample) instead of two dependent ones;
-//   FO_NEXT_SAMPLE  (with FO_NEXT_ID) the next tile's sample is also fetched, after L3, so a tile starts on no global load.
+//   FO_NEXT_SAMPLE  (with FO_NEXT_ID) the next tile's sample is also fetched, after L3, so a tile starts on no global load;
+//   FO_PIPE         two tiles in flight per warpgroup (the other bits do not apply): layers 1-3 take their A operand from
+//                   registers, so the activation tile is free from the end of L0 until the L3 rows are staged, and the row threads
+//                   build the next tile's layer-0 input there while the tensor cores run this tile's L1-L3.
 // Each holds registers across the wgmma chain, and for some instantiations that makes ptxas serialise the chain's wgmma
-// instructions (warnings C7511 / C7520).  The table gives each instantiation the first of 7, 3, 6, 1, 2, 0 with which ptxas (CUDA
-// 12.9, -Xptxas -v) builds it without C7511, C7520 or spills; every front instantiation compiles without them.  One digit per
-// pair count NP = 1 .. 16.
-constexpr int FO_F8_EARLY = 1, FO_NEXT_ID = 2, FO_NEXT_SAMPLE = 4;
+// instructions (warnings C7511 / C7513 / C7520).  The table gives each instantiation the first of 8, 7, 3, 6, 1, 2, 0 with which ptxas
+// (CUDA 12.9, -Xptxas -v) builds it without C7511, C7513, C7520 or spills; every front instantiation compiles without them.  One digit
+// per pair count NP = 1 .. 16.
+constexpr int FO_F8_EARLY = 1, FO_NEXT_ID = 2, FO_NEXT_SAMPLE = 4, FO_PIPE = 8;
 __host__ __device__ constexpr int front_opts(int nv, int np, bool grid) {
-  const char* t = nv <= 3 ? (grid ? "7726777776337767" : "1733777773773717") : (grid ? "7777776777333771" : "7777773777173373");
+  const char* t = nv <= 3 ? (grid ? "8888888387888887" : "8888888783888887") : (grid ? "8888888787888886" : "8888888787888887");
   return t[np - 1] - '0';
 }
 
@@ -447,7 +565,6 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
   constexpr int NK = 2 * NP, FWG = front_wgs(NK, NV), SPW = spw(NV), FSPT = fspt(NV);
   constexpr TcPlan plan = make_tc_plan(NK);
   constexpr uint32_t WBYTES = plan.st[4].off;        // W_hi of stages 0..3
-  constexpr int PA = tc_l0_pa(NK), FA = tc_l0_fa(NK);
   const long long end = min((long long)*count_ptr, base + len);
   if (end <= base) return;
   const int ntiles = (int)((end - base + FSPT - 1) / FSPT);
@@ -461,126 +578,138 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
   float* D3 = reinterpret_cast<float*>(A);
   const uint32_t W = tc::smem_u32(wsm);
   const int bar_id = 1 + wg;
-  const int row = (wq & 1) * 32 + lane, h = wq >> 1;
+  // row warps 2 rh and 2 rh + 1 hold rows 32 rh .. 32 rh + 31 (lane = row) with column half h = 0 and 1, so that the 16 rows of a
+  // warp's wgmma fragments (16 wq .. 16 wq + 15) are rows of its own lanes
+  const int rh = wq >> 1, h = wq & 1;
+  const int row = rh * 32 + lane;
   const int g = lane / NV, v = lane - NV * g;         // 3 views: lanes 30, 31 replay views 0, 1 of the warp's last sample (unused)
   const Group<NV> grp(lane);
   const int tile0 = blockIdx.x * FWG + wg, tstride = gridDim.x * FWG;
-  const long long srow = (wq & 1) * SPW + min(g, SPW - 1);   // this lane's sample within a tile
+  const long long srow = rh * SPW + min(g, SPW - 1);   // this lane's sample within a tile
   constexpr int OPT = front_opts(NV, NP, GRID);
-  constexpr bool F8_EARLY = (OPT & FO_F8_EARLY) != 0, NEXT_ID = (OPT & FO_NEXT_ID) != 0;
-  constexpr bool NEXT_SAMPLE = NEXT_ID && (OPT & FO_NEXT_SAMPLE) != 0;
-  // the tile ahead's work-list entry (and sample) are fetched while the current tile runs; past the end the fetch is clamped to
-  // the last entry and not used
-  int idn = 0;
-  float pn[3] = {0.0f, 0.0f, 0.0f};
-  if constexpr (NEXT_ID) {
-    idn = list[min(base + (long long)tile0 * FSPT + srow, end - 1)];
-    if constexpr (NEXT_SAMPLE) {
-      float dd[3];
-      fetch_sample<GRID>(src, idn, pn, dd);
-    }
-  }
-  for (int tile = tile0; tile < ntiles; tile += tstride) {
-    const long long si = base + (long long)tile * FSPT + srow;
+  if constexpr ((OPT & FO_PIPE) != 0) {
+    // ---- two tiles in flight.  Per tile: L0 from the activation tile (then free); the previous tile's L3 rows staged there and
+    //      pooled; L1 -> L2 -> L3 from registers, each issued before the row threads build a part of the next tile's layer-0 input
+    //      in the free tile (sample | view weight and feat8 words | encodings and feat64) and retired after it.  The work-list
+    //      entry of the tile after next is loaded beside L3, so the sample fetch beside L1 is one global load.  The tile's L3
+    //      accumulators and view weight wait in registers across the next tile's L0.
+    int tile = tile0;
+    if (tile >= ntiles) return;
     float p[3];
-    if constexpr (NEXT_SAMPLE) {
-      p[0] = pn[0]; p[1] = pn[1]; p[2] = pn[2];
-    } else {
-      float dd[3];
-      fetch_sample<GRID>(src, NEXT_ID ? idn : list[min(si, end - 1)], p, dd);
-    }
-    if constexpr (NEXT_ID) idn = list[min(si + (long long)tstride * FSPT, end - 1)];
-    const Proj q = project_s(scs, v, p);
-    const float bw = boundary_weight_fast(q);
-    const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
-    uint32_t f8w[2];
-    if constexpr (F8_EARLY) gather_feat8(scs, v, q, h, f8w);
-    // ---- stage 0 input (reference src/spatial.py:63-118 encoding | src/utils.py:74-89 feat64 gather), column order tc_kmap:
-    //      this thread writes the encodings of its run (and thread 1 the bias column and K padding), gather_feat64 the feat64
-    //      words of both runs
+    Proj q;
+    float pw;
+    uint32_t f8[2];
     {
-      float c[3];
-      const float* E = scs.E[v];
-      c[0] = E[0] * p[0] + E[1] * p[1] + E[2] * p[2] + E[3];
-      c[1] = E[4] * p[0] + E[5] * p[1] + E[6] * p[2] + E[7];
-      c[2] = E[8] * p[0] + E[9] * p[1] + E[10] * p[2] + E[11];
-      gather_feat64<NV, NP>(scs.f64, make_taps(q.u, q.v, scs.f64.W, scs.f64.H), A, (wq & 1) * 32, h, lane);
-      constexpr int C1 = 7 * PA + FA / 2;             // thread 0's run: words [0, C1); thread 1's: [C1, K0P / 2)
-      static_assert(C1 % 4 == 0 && C1 > 0, "both runs start on a 16-byte chunk");
-      if (h == 0) {
-        if constexpr (PA > 0) {
-          uint32_t a[7 * PA];
-#pragma unroll
-          for (int j = 0; j < PA; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * j);
-          a_put_span<0, 7 * PA>(A, row, a);
-        }
-      } else {
-        constexpr int NE = 7 * (NP - PA), NF = (64 - FA) / 2;
-        constexpr int N1 = tc_k0p(NK) / 2 - C1;
-        static_assert(NE + NF + 1 <= N1, "the bias column is in thread 1's run");
-        uint32_t a[NE > 0 ? NE : 1];
-#pragma unroll
-        for (int j = PA; j < NP; ++j) encode_pair<NP, NV>(scs, v, j, nk, c, a + 7 * (j - PA));
-        if constexpr (NE > 0) a_put_span<C1, NE>(A, row, a);
-        uint32_t b[N1 - NE - NF];
-        b[0] = H2_ONE;
-#pragma unroll
-        for (int i = 1; i < N1 - NE - NF; ++i) b[i] = 0u;
-        a_put_span<C1 + NE + NF, N1 - NE - NF>(A, row, b);
-      }
-    }
-    // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720)
-    float d[64];
-    front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
-    front_epi_sp(d, A, wq, lane, false);
-    if (h == 0) {   // layer-1 input: bias chunk
-      const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-      a_put<64, 8>(A, row, 64, b);
-    }
-    front_mma<128, 9>(d, A, W + plan.st[1].off, bar_id);
-    front_epi_sp(d, A, wq, lane, false);
-    {   // layer-2 input: feat8 (words 64 + 2h, 65 + 2h from this thread) | bias chunk (thread 1)
-      if constexpr (!F8_EARLY) gather_feat8(scs, v, q, h, f8w);
-      const uint32_t b[6] = {f8w[0], f8w[1], H2_ONE, 0u, 0u, 0u};
-      if (h == 0) a_put_span<64, 2>(A, row, b);
-      else a_put_span<66, 6>(A, row, b);
-    }
-    front_mma<128, 9>(d, A, W + plan.st[2].off, bar_id);
-    front_epi_sp(d, A, wq, lane, true);
-    front_mma<64, 8>(d, A, W + plan.st[3].off, bar_id);
-    if constexpr (NEXT_SAMPLE) {   // the next tile's sample (its work-list entry was loaded above)
       float dd[3];
-      fetch_sample<GRID>(src, idn, pn, dd);
+      fetch_sample<GRID>(src, list[min(base + (long long)tile * FSPT + srow, end - 1)], p, dd);
+      q = project_s(scs, v, p);
+      const float bw = boundary_weight_fast(q);
+      pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
+      gather_feat8_frag(scs, q, wq, lane, f8);
+      gather_feat64<NV, NP>(scs.f64, make_taps(q.u, q.v, scs.f64.W, scs.f64.H), A, rh * 32, h, lane);
+      front_l0_encode<NV, NP>(scs, v, nk, p, A, row, h);
     }
-    // ---- L3 rows and the rows' view weights to shared memory (over the dead activation tile), then the view pooling: weighted
-    //      mean || variance over the NV rows of a sample (src/utils.py:722-748), one (sample, 4 columns) item per thread at a time
-#pragma unroll
-    for (int m = 0; m < 16; ++m) {
-      const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 8 * (m >> 1) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(D3 + r * D3S + c) = make_float2(d[2 * m], d[2 * m + 1]);
-    }
-    if (h == 0) D3[64 * D3S + row] = pw;
-    tc::named_sync(bar_id, 128);
-    for (int it = t & 127; it < FSPT * 16; it += 128) {
-      const int s = it >> 4, c = 4 * (it & 15);
-      const int r0 = (s / SPW) * 32 + NV * (s % SPW);   // row of the sample's view 0
-      float4 x[NV];
-      float w[NV];
-#pragma unroll
-      for (int u = 0; u < NV; ++u) {
-        x[u] = *reinterpret_cast<const float4*>(D3 + (r0 + u) * D3S + c);
-        w[u] = D3[64 * D3S + r0 + u];
+    const uint32_t k8_bias = (lane & 3) == 0 ? H2_ONE : 0u;   // bias word at column 0 of a k-block's word group, K padding after
+    float d[64];
+    uint32_t a[36];
+    front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
+    front_sp_frag(d, a);
+    float d3[32];
+    int idn = list[min(base + (long long)(tile + tstride) * FSPT + srow, end - 1)];
+    for (;;) {
+      // the next tile's input is built whether or not there is one (past the end the work-list index is clamped), so that no
+      // branch separates a wgmma chain from its wait
+      const int next = tile + tstride;
+      a[32] = k8_bias; a[33] = k8_bias; a[34] = 0u; a[35] = 0u;   // layer-1 input words 64..71: bias column, K padding
+      front_ra_issue<128, 9>(d, a, W + plan.st[1].off);
+      float pwn;
+      uint32_t f8n[2];
+      {
+        float dd[3];
+        fetch_sample<GRID>(src, idn, p, dd);
       }
-      float4 mn, vr;
-      pool_views<NV>(w, x, mn, vr);
-      const long long sj = base + (long long)tile * FSPT + s;
-      if (sj < end) {
-        float* out = pool + (sj - base) * POOL_W + c;
-        *reinterpret_cast<float4*>(out) = mn;
-        *reinterpret_cast<float4*>(out + 64) = vr;
+      front_ra_wait<128>(d);
+      front_sp_frag(d, a);
+      a[32] = f8[0]; a[33] = f8[1]; a[34] = k8_bias; a[35] = k8_bias;   // layer-2 input words 64..71: feat8 | bias, K padding
+      front_ra_issue<128, 9>(d, a, W + plan.st[2].off);
+      {
+        q = project_s(scs, v, p);
+        const float bw = boundary_weight_fast(q);
+        pwn = bw / (grp.sum(bw) + 1e-6f);
+        gather_feat8_frag(scs, q, wq, lane, f8n);
+      }
+      front_ra_wait<128>(d);
+      front_sp_frag(d, a);
+      a[30] = k8_bias; a[31] = k8_bias;   // layer-3 input words 60..63: bias column, K padding
+      front_ra_issue<64, 8>(d3, a, W + plan.st[3].off);
+      front_l0_encode<NV, NP>(scs, v, nk, p, A, row, h);
+      gather_feat64<NV, NP>(scs.f64, make_taps(q.u, q.v, scs.f64.W, scs.f64.H), A, rh * 32, h, lane);
+      idn = list[min(base + (long long)(next + tstride) * FSPT + srow, end - 1)];
+      front_ra_wait<64>(d3);
+      if (next >= ntiles) break;
+      front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
+      front_sp_frag(d, a);
+      front_pool<NV>(d3, pw, D3, wq, lane, row, h, base, end, tile, pool, bar_id);
+      tile = next; pw = pwn; f8[0] = f8n[0]; f8[1] = f8n[1];
+    }
+    tc::named_sync(bar_id, 128);   // every thread's writes of the unused input are done before the L3 rows go over them
+    front_pool<NV>(d3, pw, D3, wq, lane, row, h, base, end, tile, pool, bar_id);
+  } else {
+    constexpr bool F8_EARLY = (OPT & FO_F8_EARLY) != 0, NEXT_ID = (OPT & FO_NEXT_ID) != 0;
+    constexpr bool NEXT_SAMPLE = NEXT_ID && (OPT & FO_NEXT_SAMPLE) != 0;
+    // the tile ahead's work-list entry (and sample) are fetched while the current tile runs; past the end the fetch is clamped to
+    // the last entry and not used
+    int idn = 0;
+    float pn[3] = {0.0f, 0.0f, 0.0f};
+    if constexpr (NEXT_ID) {
+      idn = list[min(base + (long long)tile0 * FSPT + srow, end - 1)];
+      if constexpr (NEXT_SAMPLE) {
+        float dd[3];
+        fetch_sample<GRID>(src, idn, pn, dd);
       }
     }
-    tc::named_sync(bar_id, 128);   // the L3 rows are read: the next tile's input may overwrite them
+    for (int tile = tile0; tile < ntiles; tile += tstride) {
+      const long long si = base + (long long)tile * FSPT + srow;
+      float p[3];
+      if constexpr (NEXT_SAMPLE) {
+        p[0] = pn[0]; p[1] = pn[1]; p[2] = pn[2];
+      } else {
+        float dd[3];
+        fetch_sample<GRID>(src, NEXT_ID ? idn : list[min(si, end - 1)], p, dd);
+      }
+      if constexpr (NEXT_ID) idn = list[min(si + (long long)tstride * FSPT, end - 1)];
+      const Proj q = project_s(scs, v, p);
+      const float bw = boundary_weight_fast(q);
+      const float pw = bw / (grp.sum(bw) + 1e-6f);   // reference src/model.py:750-759 (mask == 1 for shaded samples)
+      uint32_t f8w[2];
+      if constexpr (F8_EARLY) gather_feat8(scs, v, q, h, f8w);
+      gather_feat64<NV, NP>(scs.f64, make_taps(q.u, q.v, scs.f64.W, scs.f64.H), A, rh * 32, h, lane);
+      front_l0_encode<NV, NP>(scs, v, nk, p, A, row, h);
+      // ---- L0 -> L1 -> L2 -> L3 (reference src/utils.py:691-720)
+      float d[64];
+      front_mma<128, tc_k0p(NK) / 16>(d, A, W + plan.st[0].off, bar_id);
+      front_epi_sp(d, A, wq, lane, false);
+      if (h == 0) {   // layer-1 input: bias chunk
+        const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+        a_put<64, 8>(A, row, 64, b);
+      }
+      front_mma<128, 9>(d, A, W + plan.st[1].off, bar_id);
+      front_epi_sp(d, A, wq, lane, false);
+      {   // layer-2 input: feat8 (words 64 + 2h, 65 + 2h from this thread) | bias chunk (thread 1)
+        if constexpr (!F8_EARLY) gather_feat8(scs, v, q, h, f8w);
+        const uint32_t b[6] = {f8w[0], f8w[1], H2_ONE, 0u, 0u, 0u};
+        if (h == 0) a_put_span<64, 2>(A, row, b);
+        else a_put_span<66, 6>(A, row, b);
+      }
+      front_mma<128, 9>(d, A, W + plan.st[2].off, bar_id);
+      front_epi_sp(d, A, wq, lane, true);
+      front_mma<64, 8>(d, A, W + plan.st[3].off, bar_id);
+      if constexpr (NEXT_SAMPLE) {   // the next tile's sample (its work-list entry was loaded above)
+        float dd[3];
+        fetch_sample<GRID>(src, idn, pn, dd);
+      }
+      front_pool<NV>(d, pw, D3, wq, lane, row, h, base, end, tile, pool, bar_id);
+    }
   }
 }
 

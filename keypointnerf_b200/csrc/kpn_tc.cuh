@@ -1,5 +1,5 @@
-// Thin inline-PTX layer over the sm_90a tensor-core path: warpgroup MMA (wgmma.mma_async, both operands in shared memory
-// through matrix descriptors, fp32 accumulators in registers), mbarrier and the 1-D bulk (TMA) copy.  Encodings follow the
+// Thin inline-PTX layer over the sm_90a tensor-core path: warpgroup MMA (wgmma.mma_async, B and usually A in shared memory
+// through matrix descriptors, A also from registers, fp32 accumulators in registers), mbarrier and the 1-D bulk (TMA) copy.  Encodings follow the
 // PTX ISA wgmma chapter; the bit layout of the shared-memory descriptor is restated below.
 #pragma once
 #include <cuda_fp16.h>
@@ -101,6 +101,19 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Pins N registers in program order between the volatile wgmma statements: a register-A fragment fenced before wg_fence() is
+// complete before the chain starts (the compiler would otherwise sink its last definitions between the chain's MMAs, and ptxas
+// then serialises them, C7513), and accumulators fenced after wg_wait0() are not read before the wait.
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
 
 }  // namespace tc
 }  // namespace kpn
@@ -124,6 +137,15 @@ __device__ __forceinline__ void wg_mma(float* d, uint32_t a_addr, uint32_t a_lbo
   for (int j = 0; j < KCH; ++j)
     Wgmma<N>::mma(d, make_smem_desc(a_addr + 2u * a_lbo * (uint32_t)j, a_lbo, 128u),
                   make_smem_desc(b_addr + 2u * b_lbo * (uint32_t)j, b_lbo, 128u), (acc || j > 0) ? 1u : 0u);
+}
+
+// The same product with A from registers: a[4j .. 4j + 3] is k-block j's fragment (WgmmaRA).  The registers must stay unchanged
+// until the caller's wg_wait0() after the chain.
+template <int N, int KCH>
+__device__ __forceinline__ void wg_mma_ra(float* d, const uint32_t* a, uint32_t b_addr, uint32_t b_lbo, uint32_t acc) {
+#pragma unroll
+  for (int j = 0; j < KCH; ++j)
+    WgmmaRA<N>::mma(d, a + 4 * j, make_smem_desc(b_addr + 2u * b_lbo * (uint32_t)j, b_lbo, 128u), (acc || j > 0) ? 1u : 0u);
 }
 
 // named barriers (ids 1..15): producer arrives, consumer syncs; `count` = threads of both sides
