@@ -48,107 +48,154 @@ colour_list_kernel(const int* __restrict__ list, const int* __restrict__ count_p
 
 // =====================================================================================================================
 // geometry tail: P0|compress and P1 per sample (64 samples per warpgroup tile, two threads per row for the input build),
-// two-term weights and activations: D = A_hi W_hi [+ A_hi W_lo] [+ A_lo W_hi] (lo_mask bits 4/5: W_lo of stage 4/5,
-// bits 6/7: A_lo of stage 4/5).  Everything after the input build runs on the accumulator fragments.
+// two-term weights and activations: D = A_hi W_hi [+ A_hi W_lo] [+ A_lo W_hi] (LO_MASK bits 4/5: W_lo of stage 4/5, bits 6/7:
+// A_lo of stage 4/5).  A tile's pooled rows arrive in the warpgroup's staging slot by one bulk copy, issued while the tile before
+// it runs its MMAs; P0|compress reads its input tiles from shared memory, P1 takes its A operand from registers (P0's
+// accumulator fragments after the softplus).  Everything after the input build runs on the accumulator fragments.
 // =====================================================================================================================
-constexpr uint32_t T4H = 64 * 144 * 2, T4L = 64 * 128 * 2, T5H = 64 * 80 * 2, T5L = 64 * 64 * 2;   // activation tiles
-constexpr uint32_t TAIL_TILE_BYTES = T4H + T4L + T5H + T5L;
+constexpr uint32_t T4H = 64 * 144 * 2, T4L = 64 * 128 * 2;   // P0|compress input tiles: [mean hi | var hi | bias chunk], [mean lo | var lo]
+constexpr uint32_t TAIL_SLOT = 64 * POOL_W * 4;              // staging slot: the pooled rows of one tile
+constexpr uint32_t TAIL_WG_BYTES = T4H + T4L + TAIL_SLOT;
+constexpr uint32_t tail_smem_bytes() {
+  return 2 * (REL_PLAN.st[GEO_NSTAGE].off - REL_PLAN.st[4].off) + GWG * TAIL_WG_BYTES;
+}
+static_assert(tail_smem_bytes() == 210944u && tail_smem_bytes() + 1024u <= SMEM_OPTIN,
+              "W_hi + W_lo of stages 4-5 and two warpgroups' input tiles and staging slots fit beside the static block");
 
-template <int N, int KH, int KL>
-__device__ __forceinline__ void tail_mma(float* d, const uint8_t* ahi, const uint8_t* alo, uint32_t whi, uint32_t wlo, bool w_lo,
-                                         bool a_lo, int bar_id) {
+// One sub-chain sequence of a tail stage, committed once: A_hi W_hi (KH k-blocks), then A_hi W_lo, then A_lo W_hi (KL k-blocks),
+// into the same accumulators.  A from shared memory (the activation tiles ahi / alo).
+template <int N, int KH, int KL, bool W_LO, bool A_LO>
+__device__ __forceinline__ void tail_mma(float* d, const uint8_t* ahi, const uint8_t* alo, uint32_t whi, uint32_t wlo) {
   constexpr uint32_t lbo = (uint32_t)(N / 8) * 128u;
-  wg_publish(bar_id);
   tc::wg_fence();
   tc::wg_mma<N, KH>(d, tc::smem_u32(ahi), 1024u, whi, lbo, 0u);
-  if (w_lo) tc::wg_mma<N, KH>(d, tc::smem_u32(ahi), 1024u, wlo, lbo, 1u);
-  if (a_lo) tc::wg_mma<N, KL>(d, tc::smem_u32(alo), 1024u, whi, lbo, 1u);
+  if constexpr (W_LO) tc::wg_mma<N, KH>(d, tc::smem_u32(ahi), 1024u, wlo, lbo, 1u);
+  if constexpr (A_LO) tc::wg_mma<N, KL>(d, tc::smem_u32(alo), 1024u, whi, lbo, 1u);
   tc::wg_commit();
   tc::wg_wait0();
-  tc::named_sync(bar_id, 128);
+  tc::fence_regs<N / 2>(d);
+}
+// The same with A from registers: ahi[4 KH], alo[4 KL] (the k-block fragments of WgmmaRA).
+template <int N, int KH, int KL, bool W_LO, bool A_LO>
+__device__ __forceinline__ void tail_mma_ra(float* d, uint32_t* ahi, uint32_t* alo, uint32_t whi, uint32_t wlo) {
+  constexpr uint32_t lbo = (uint32_t)(N / 8) * 128u;
+  tc::fence_regs<4 * KH>(ahi);
+  if constexpr (A_LO) tc::fence_regs<4 * KL>(alo);
+  tc::fence_regs<N / 2>(d);
+  tc::wg_fence();
+  tc::wg_mma_ra<N, KH>(d, ahi, whi, lbo, 0u);
+  if constexpr (W_LO) tc::wg_mma_ra<N, KH>(d, ahi, wlo, lbo, 1u);
+  if constexpr (A_LO) tc::wg_mma_ra<N, KL>(d, alo, whi, lbo, 1u);
+  tc::wg_commit();
+  tc::wg_wait0();
+  tc::fence_regs<N / 2>(d);
 }
 
 // whi: the blob's W_hi tile of stage 4 (stage 5's follows it).  GEO_ONLY: the geometry-only query (query_mode 2), which writes
-// so.out2 and keeps no latent; a template parameter, so that the render / query instantiation is unchanged.
-template <bool GEO_ONLY>
+// so.out2 and keeps no latent.  LO_MASK: the W_lo / A_lo sub-chains (0xF0 two-term weights, 0xC0 single-term: kpn_api.cu); a
+// template parameter, so that each stage's chain is one branch-free wgmma sequence.
+template <bool GEO_ONLY, int LO_MASK>
 __global__ void __launch_bounds__(GWG * 128, 1)
-geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ whi, const uint8_t* __restrict__ wlo, int lo_mask,
+geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ whi, const uint8_t* __restrict__ wlo,
                 const int* __restrict__ list, const int* __restrict__ count_ptr, long long base, long long len,
                 const float* __restrict__ pool, int query_mode, ShadeOut so, uint4* __restrict__ lat_out) {
   extern __shared__ __align__(1024) uint8_t wsm[];
-  __shared__ uint64_t wbar;
+  __shared__ uint64_t wbar, sbar[GWG];                     // weights; each warpgroup's staging slot
   __shared__ __align__(16) float wp2[132];                 // density head: w[0][64] | w[1][64] | b[2]
   constexpr TcPlan plan = REL_PLAN;
   constexpr uint32_t HOFF = plan.st[4].off, WH = plan.st[GEO_NSTAGE].off - plan.st[4].off;   // W_hi of stages 4, 5
+  constexpr bool W_LO4 = (LO_MASK >> 4) & 1, W_LO5 = (LO_MASK >> 5) & 1, A_LO4 = (LO_MASK >> 6) & 1, A_LO5 = (LO_MASK >> 7) & 1;
   const long long end = min((long long)*count_ptr, base + len);
   if (end <= base) return;
   const int ntiles = (int)((end - base + 63) / 64);
   const int t = threadIdx.x, wg = t >> 7, wt = t & 127, wq = wt >> 5, lane = t & 31;
+  const int tstride = gridDim.x * GWG;
+  auto slot_of = [&](int w) { return reinterpret_cast<float*>(wsm + 2 * WH + (size_t)w * TAIL_WG_BYTES + T4H + T4L); };
+  // the pooled rows of a tile are contiguous in the scratch: one bulk copy of its valid rows into warpgroup w's slot
+  auto stage_rows = [&](int w, int tile) {
+    const long long s0 = (long long)tile * 64;
+    const uint32_t bytes = (uint32_t)min(64ll, end - base - s0) * (POOL_W * 4u);
+    tc::mbar_expect_tx(&sbar[w], bytes);
+    tc::bulk_g2s(slot_of(w), pool + s0 * POOL_W, bytes, &sbar[w]);
+  };
   for (int i = t; i < 130; i += GWG * 128) wp2[i] = i < 64 ? C.w_p2[0][i] : i < 128 ? C.w_p2[1][i - 64] : C.b_p2[i - 128];
-  if (t == 0) { tc::mbar_init(&wbar, 1); tc::fence_mbar_init(); }
+  if (t == 0) {
+    tc::mbar_init(&wbar, 1);
+    for (int w = 0; w < GWG; ++w) tc::mbar_init(&sbar[w], 1);
+    tc::fence_mbar_init();
+  }
   __syncthreads();
-  if (t == 0) {   // [W_hi 4 | W_hi 5 | W_lo 4 | W_lo 5]
+  if (t == 0) {   // [W_hi 4 | W_hi 5 | W_lo 4 | W_lo 5], then each warpgroup's first tile
     tc::mbar_expect_tx(&wbar, 2 * WH);
     tc::bulk_g2s(wsm, whi, WH, &wbar);
     tc::bulk_g2s(wsm + WH, wlo, WH, &wbar);
+    for (int w = 0; w < GWG; ++w)
+      if (blockIdx.x * GWG + w < ntiles) stage_rows(w, blockIdx.x * GWG + w);
     tc::mbar_wait(&wbar, 0, 0x31u);
   }
   __syncthreads();
-  uint8_t* A4h = wsm + 2 * WH + (size_t)wg * TAIL_TILE_BYTES;
+  uint8_t* A4h = wsm + 2 * WH + (size_t)wg * TAIL_WG_BYTES;
   uint8_t* A4l = A4h + T4H;
-  uint8_t* A5h = A4l + T4L;
-  uint8_t* A5l = A5h + T5H;
+  const float* slot = slot_of(wg);
   const uint32_t W4h = tc::smem_u32(wsm), W5h = W4h + (plan.st[5].off - HOFF), W4l = W4h + WH, W5l = W5h + WH;
   const int bar_id = 1 + wg;
   const int row = wt & 63, h = wt >> 6;
-  if (h == 0) {   // bias chunks of the two stages' inputs (never overwritten)
+  if (h == 0) {   // bias chunk of P0's input (never overwritten)
     const uint32_t b[8] = {H2_ONE, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
     a_put<64, 8>(A4h, row, 64, b);
-    a_put<64, 8>(A5h, row, 32, b);
   }
-  for (int tile = blockIdx.x * GWG + wg; tile < ntiles; tile += gridDim.x * GWG) {
+  // P1's input words 64..71 (k-block 4): bias column, K padding
+  const uint32_t k_bias = (lane & 3) == 0 ? H2_ONE : 0u;
+  // the 8 threads of a quarter warp hold 8 consecutive rows, 512 bytes apart in the slot: each reads the 32-byte pairs of its
+  // half-row rotated by its row (pair p + row, first or second 16 bytes first), so that the 8 reads of a quarter warp fall in
+  // 8 different 16-byte bank groups
+  const int rot = row & 3, sw = (row >> 2) & 1;
+  int phase = 0;
+  for (int tile = blockIdx.x * GWG + wg; tile < ntiles; tile += tstride, phase ^= 1) {
     const long long t0 = base + (long long)tile * 64;
-    {   // P0|compress input: [mean hi | var hi | bias chunk], [mean lo | var lo]
-      const long long si = min(t0 + row, end - 1);
-      const float* in = pool + (si - base) * POOL_W + 32 * h;
-      uint32_t mh[16], ml[16], vh[16], vl[16];
+    tc::mbar_wait(&sbar[wg], (uint32_t)phase, 0x32u);
+    {   // P0|compress input: [mean hi | var hi | bias chunk], [mean lo | var lo]; the ghost rows of a partial tile repeat the
+        // last valid row (they are never written)
+      const float4* in = reinterpret_cast<const float4*>(slot + (size_t)min((long long)row, end - 1 - t0) * POOL_W + 32 * h);
 #pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4) {
-        const float4 m = __ldg(reinterpret_cast<const float4*>(in) + c4);
-        const float4 s = __ldg(reinterpret_cast<const float4*>(in + 64) + c4);
-        split_h2(m.x, m.y, mh[2 * c4], ml[2 * c4]);
-        split_h2(m.z, m.w, mh[2 * c4 + 1], ml[2 * c4 + 1]);
-        split_h2(s.x, s.y, vh[2 * c4], vl[2 * c4]);
-        split_h2(s.z, s.w, vh[2 * c4 + 1], vl[2 * c4 + 1]);
-      }
-      a_put<64, 16>(A4h, row, 16 * h, mh);
-      a_put<64, 16>(A4h, row, 32 + 16 * h, vh);
-      a_put<64, 16>(A4l, row, 16 * h, ml);
-      a_put<64, 16>(A4l, row, 32 + 16 * h, vl);
-    }
-    // ---- P0 (softplus, two fp16 terms out) | compress (linear, fp16 latent kept in registers until the density is known)
-    uint32_t lat[2][3];
-    {
-      float d[48];
-      tail_mma<96, 9, 8>(d, A4h, A4l, W4h, W4l, (lo_mask >> 4) & 1, (lo_mask >> 6) & 1, bar_id);
+      for (int half = 0; half < 2; ++half) {   // mean, var
 #pragma unroll
-      for (int m = 0; m < 24; ++m) {
-        const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);
-        if (m < 16) {
-          uint32_t hi, lo;
-          split_h2(sp_fast(d[2 * m]), sp_fast(d[2 * m + 1]), hi, lo);
-          a_word(A5h, r, c, hi);
-          a_word(A5l, r, c, lo);
-        } else if (m < 22) {
-          lat[m & 1][(m >> 1) - 8] = tc::pack_h2(d[2 * m], d[2 * m + 1]);
+        for (int p = 0; p < 4; ++p) {
+          const int q = (p + rot) & 3;
+          const float4 u = in[16 * half + 2 * q + sw], v = in[16 * half + 2 * q + 1 - sw];
+          const float4 x0 = sw ? v : u, x1 = sw ? u : v;   // floats 8q .. 8q + 7 of the half-row
+          uint32_t hi[4], lo[4];
+          split_h2(x0.x, x0.y, hi[0], lo[0]);
+          split_h2(x0.z, x0.w, hi[1], lo[1]);
+          split_h2(x1.x, x1.y, hi[2], lo[2]);
+          split_h2(x1.z, x1.w, hi[3], lo[3]);
+          a_put<64, 4>(A4h, row, 32 * half + 16 * h + 4 * q, hi);
+          a_put<64, 4>(A4l, row, 32 * half + 16 * h + 4 * q, lo);
         }
       }
     }
+    wg_publish(bar_id);   // the input tiles are visible to the MMAs, and every thread of the warpgroup is done with the slot
+    if (wt == 0 && tile + tstride < ntiles) stage_rows(wg, tile + tstride);
+    // ---- P0 (softplus, two fp16 terms out: P1's A fragments) | compress (linear, fp16 latent kept in registers until the
+    //      density is known).  a*[m] is the word at row 16 wq + (lane >> 2) + 8 (m & 1), word column 4 (m >> 1) + (lane & 3), so
+    //      a*[4j .. 4j + 3] is k-block j of P1's input.
+    uint32_t ahi[20], alo[16], lat[2][3];
+    {
+      float d[48];
+      tail_mma<96, 9, 8, W_LO4, A_LO4>(d, A4h, A4l, W4h, W4l);
+      tc::named_sync(bar_id, 128);   // the input tiles are read: the next tile's may overwrite them
+#pragma unroll
+      for (int m = 0; m < 24; ++m) {
+        if (m < 16) split_h2(sp_fast(d[2 * m]), sp_fast(d[2 * m + 1]), ahi[m], alo[m]);
+        else if (m < 22) lat[m & 1][(m >> 1) - 8] = tc::pack_h2(d[2 * m], d[2 * m + 1]);
+      }
+    }
+    ahi[16] = k_bias; ahi[17] = k_bias; ahi[18] = 0u; ahi[19] = 0u;
     // ---- P1 (softplus) then the 64->2 density head in fp32: partial dots over this lane's 16 columns, summed over the quad
     float gs[2] = {0.0f, 0.0f}, rs[2] = {0.0f, 0.0f};
     {
       float d[32];
-      tail_mma<64, 5, 4>(d, A5h, A5l, W5h, W5l, (lo_mask >> 5) & 1, (lo_mask >> 7) & 1, bar_id);
+      tail_mma_ra<64, 5, 4, W_LO5, A_LO5>(d, ahi, alo, W5h, W5l);
 #pragma unroll
       for (int m = 0; m < 16; ++m) {
         const int c = 8 * (m >> 1) + 2 * (lane & 3);
@@ -161,19 +208,20 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
     //      alpha == 0 composites with weight exactly 0, skipping its colour is exact; every valid sample in query mode; none in
     //      geometry-only mode), the compressed latent at the sample's own list index
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      float g0 = gs[k], rad = rs[k];
+    for (int m = 0; m < 2; ++m) {   // the quad's rows: fragment pairs 0 and 1, row r, word column c (the latent word of the lane)
+      const int r = 16 * wq + (lane >> 2) + 8 * (m & 1), c = 4 * (m >> 1) + (lane & 3);
+      float g0 = gs[m], rad = rs[m];
       g0 += __shfl_xor_sync(FULL, g0, 1); g0 += __shfl_xor_sync(FULL, g0, 2);
       rad += __shfl_xor_sync(FULL, rad, 1); rad += __shfl_xor_sync(FULL, rad, 2);
       g0 += wp2[128];
       rad += wp2[129];
-      const long long si = t0 + 16 * wq + (lane >> 2) + 8 * k;
+      const long long si = t0 + r;
       if (si < end) {
         if (GEO_ONLY) {
-          if ((lane & 3) == 0) reinterpret_cast<float2*>(so.out2)[list[si]] = make_float2(g0, rad);
+          if (c == 0) reinterpret_cast<float2*>(so.out2)[list[si]] = make_float2(g0, rad);
           continue;
         }
-        if ((lane & 3) == 0) {
+        if (c == 0) {
           if (query_mode) {
             float* o = so.out5 + 5ll * list[si];
             o[0] = g0; o[1] = rad; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f;
@@ -184,7 +232,7 @@ geo_tail_kernel(const __grid_constant__ TcConsts C, const uint8_t* __restrict__ 
         if (query_mode != 0 || rad > 0.0f) {
           uint32_t* lw = reinterpret_cast<uint32_t*>(lat_out + 3ll * si);
 #pragma unroll
-          for (int j = 0; j < 3; ++j) lw[4 * j + (lane & 3)] = lat[k][j];
+          for (int j = 0; j < 3; ++j) lw[4 * j + c] = lat[m][j];
         }
       }
     }
@@ -206,20 +254,26 @@ bool tc_supported(int n_views, int n_kpt, int sp_level) {
 cudaError_t launch_geo_tail(const TcConsts& C, const uint8_t* wtail, const uint8_t* wlo, int lo_mask, const int* list,
                             const int* counter, long long base, long long len, const float* pool, int query_mode, const ShadeOut& so,
                             uint4* lat, int num_sms, cudaStream_t st) {
-  constexpr TcPlan rel = REL_PLAN;
-  constexpr uint32_t smem_tail = 2 * (rel.st[GEO_NSTAGE].off - rel.st[4].off) + GWG * TAIL_TILE_BYTES;
+  using TailFn = decltype(&geo_tail_kernel<false, 0xF0>);
+  // [two-term | single-term weights][render / query | geometry-only]
+  static constexpr TailFn kernels[2][2] = {{geo_tail_kernel<false, 0xF0>, geo_tail_kernel<true, 0xF0>},
+                                           {geo_tail_kernel<false, 0xC0>, geo_tail_kernel<true, 0xC0>}};
+  if (lo_mask != 0xF0 && lo_mask != 0xC0) return cudaErrorInvalidValue;
+  constexpr uint32_t smem_tail = tail_smem_bytes();
   static std::atomic<bool> attr[64];   // function attributes are per device (zero-initialised; setting them twice is harmless)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(geo_tail_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(geo_tail_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
-    if (e != cudaSuccess) return e;
+    for (const auto& row : kernels)
+      for (TailFn k : row) {
+        const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tail);
+        if (e != cudaSuccess) return e;
+      }
     if (dev >= 0 && dev < 64) attr[dev].store(true, std::memory_order_release);
   }
-  auto kernel = query_mode == 2 ? geo_tail_kernel<true> : geo_tail_kernel<false>;
-  kernel<<<tc_grid((len + 63) / 64, GWG, num_sms), GWG * 128, smem_tail, st>>>(C, wtail, wlo, lo_mask, list, counter, base, len, pool,
-                                                                              query_mode, so, lat);
+  const TailFn kernel = kernels[lo_mask == 0xC0][query_mode == 2];
+  kernel<<<tc_grid((len + 63) / 64, GWG, num_sms), GWG * 128, smem_tail, st>>>(C, wtail, wlo, list, counter, base, len, pool, query_mode,
+                                                                              so, lat);
   return cudaGetLastError();
 }
 

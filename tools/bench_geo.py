@@ -8,6 +8,11 @@ The frame is bench.py's (same seeded scene, weights and target; config 2 by defa
 summed by name and divided by --steps.  The L2 flush before each frame runs inside its own record_function range, and the
 kernels linked to it are subtracted.  The profiler adds host overhead between launches but not to the kernels' own device time.  The
 card's name, power limit and maximum SM clock are read in the same run and printed with the result (one JSON line).
+
+The line also sets geo_tail_kernel's time against the two floors its shapes give, at the H100 SXM data sheet's rates (3.35 TB/s
+HBM3, 989 TFLOP/s dense fp16; figures the card is not claimed to reach): the bytes it must move (the 512-byte pooled row of every
+valid sample in, its 8-byte alpha / sdf record and, for samples with density > 0, the 48-byte latent out) and the MMA work it
+executes (per 64-sample tile, engine 0: P0|compress 26 m64n96k16 and P1 14 m64n64k16).
 """
 from __future__ import annotations
 
@@ -25,6 +30,20 @@ CONFIGS = {2: dict(size=512, S_c=128, S_f=0, fine=False, ert=0.0),
            3: dict(size=512, S_c=64, S_f=64, fine=True, ert=1e-4),
            4: dict(size=1024, S_c=128, S_f=0, fine=False, ert=0.0)}
 GROUPS = ("geo_front_kernel", "geo_tail_kernel", "colour_list", "shade_color_kernel")
+DATASHEET_BYTES_S = 3.35e12   # H100 SXM, HBM3
+DATASHEET_FLOP_S = 989e12     # H100 SXM, dense fp16 tensor
+TAIL_TILE_FLOP = 2 * 64 * 16 * (26 * 96 + 14 * 64)   # executed MMA work of one 64-sample tile with two-term weights (engine 0)
+
+
+def tail_floors(valid: int, coloured: int, tail_ms: float) -> dict:
+    """geo_tail_kernel against the data sheet: the bytes it must move and the MMA work it executes, over its measured time."""
+    nbytes = 512 * valid + 8 * valid + 48 * coloured
+    flop = TAIL_TILE_FLOP * ((valid + 63) // 64)
+    s = tail_ms * 1e-3
+    return {"required_bytes": nbytes, "achieved_GB_s": round(nbytes / s / 1e9, 1) if s else None,
+            "datasheet_GB_s": DATASHEET_BYTES_S / 1e9, "byte_floor_ms": round(nbytes / DATASHEET_BYTES_S * 1e3, 3),
+            "executed_mma_flop": flop, "achieved_TFLOP_s": round(flop / s / 1e12, 1) if s else None,
+            "datasheet_TFLOP_s": DATASHEET_FLOP_S / 1e12, "mma_floor_ms": round(flop / DATASHEET_FLOP_S * 1e3, 3)}
 
 
 def card():
@@ -112,11 +131,13 @@ def main():
     for name, t in us.items():
         ms[group_of(name)] += (t - flush_us.get(name, 0.0)) / 1e3 / args.steps
     geo = ms["geo_front_kernel"] + ms["geo_tail_kernel"]
+    st = m.stats()
     line = {"card": card(), "config": args.config, "scene": args.scene, "n_kpt": args.n_kpt, "steps": args.steps,
-            "samples_valid": int(m.stats()["samples_valid"]),
+            "samples_valid": int(st["samples_valid"]), "samples_coloured": int(st["samples_coloured"]),
             "ms_per_frame": {k: round(v, 3) for k, v in ms.items()},
             "flush_ms_excluded": round(sum(flush_us.values()) / 1e3 / args.steps, 3),
-            "geometry_ms": round(geo, 3), "front_share_of_geometry": round(ms["geo_front_kernel"] / geo, 3) if geo else None}
+            "geometry_ms": round(geo, 3), "front_share_of_geometry": round(ms["geo_front_kernel"] / geo, 3) if geo else None,
+            "tail_vs_datasheet": tail_floors(int(st["samples_valid"]), int(st["samples_coloured"]), ms["geo_tail_kernel"])}
     m.check_health()
     print(json.dumps(line), flush=True)
     if args.out:
