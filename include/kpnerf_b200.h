@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define KPN_ABI_VERSION 4
+#define KPN_ABI_VERSION 5
 #define KPN_MAX_VIEWS 4
 #define KPN_MAX_KPT 32
 #define KPN_NUM_LAYERS 19
@@ -206,6 +206,30 @@ int kpn_render(kpn_ctx* ctx, const kpn_target* target, const kpn_opts* opts, con
  * for any subset, order or concatenation of cameras.  n == 0: KPN_OK, nothing is done; null arrays or n < 0: KPN_ERR_ARG;
  * no scene: KPN_ERR_STATE; sample counts, engines and their refusals as kpn_render. */
 int kpn_render_rays(kpn_ctx* ctx, const kpn_rays* rays, const kpn_opts* opts, const kpn_out* out, void* stream);
+
+/* Gradients of kpn_render_rays (every output a layer of the reference's hot path, mlp_tex.ani_al or a gathered feature map
+ * depends on), with the reference's autograd semantics (src/model.py:978-1096, 1150-1176, eval branch, uniform=True).  The
+ * ray batch is in the layout of kpn_render_rays; dW of layer l is (n_out, n_in) of the FOLDED weight (g * v / ||v|| for a
+ * weight-normed layer), the feature-map gradients are channel-last (V, H, W, C) with the extents of kpn_scene's maps. */
+typedef struct {
+  float* dW[KPN_NUM_LAYERS];
+  float* db[KPN_NUM_LAYERS];
+  float* d_ani_al;     /* (1) */
+  float* d_feat64;     /* (V, H, W, 64) feat_geo[0] */
+  float* d_feat8;      /* (V, H, W, 8)  feat_geo[1] */
+  float* d_feat_tex;   /* (V, H, W, 8)  feat_tex */
+  int mem;             /* kpn_mem of the pointers above */
+} kpn_grads;
+
+/* The backward of kpn_render_rays: grad_out holds dL/d of each output plane of kpn_out (same shapes; NULL plane = zero; z_fine
+ * and contrib are ignored), every array of grads is overwritten with dL/d that parameter.  The depths of the fine pass are
+ * constants (the reference resamples under torch.no_grad); source images, cameras, keypoints, bounds, rays and masks are data.
+ * The forward is recomputed with the fp32 engine whatever opts->engine says, and the gradients are fp32 (CUDA cores); the
+ * fine pass uses opts->z_fine_override when set (kpn_mem of grad_out).  Chunking as kpn_render_rays; n == 0 writes zeros.
+ * Null arrays, bad sample counts: KPN_ERR_ARG; no weights or scene: KPN_ERR_STATE; ert_eps > 0: KPN_ERR_UNSUPPORTED (the
+ * samples early-ray termination skips have gradients). */
+int kpn_render_rays_backward(kpn_ctx* ctx, const kpn_rays* rays, const kpn_opts* opts, const kpn_out* grad_out, const kpn_grads* grads,
+                             void* stream);
 
 /* The rays kpn_render marches for the target's pixel lattice, pixel j*nx+i at index j*nx+i: origins (R,3) = -t^T R,
  * dirs (R,3) = normalize(K^-1 [x,y,1] R), near_far (R,2) = |znear K^-1 [x,y,1]|, |zfar K^-1 [x,y,1]| (before the bounding-box

@@ -20,8 +20,8 @@ KPN_NHWC_FEAT64, KPN_NHWC_FEAT8, KPN_NHWC_FEATTEX = 1, 2, 4
 
 EXPORTS = ["kpn_abi_version", "kpn_create", "kpn_destroy", "kpn_last_error", "kpn_set_weights", "kpn_set_scene",
            "kpn_render", "kpn_query", "kpn_get_stats", "kpn_set_profiling", "kpn_selftest_umma", "kpn_selftest_umma2", "kpn_debug_timing", "kpn_debug_kmap", "kpn_check_health", "kpn_reserve", "kpn_debug_stage_times", "kpn_decode_views",
-           "kpn_query_grid", "kpn_mesh_begin", "kpn_mesh_emit", "kpn_render_rays", "kpn_camera_rays"]
-KPN_ABI_VERSION = 4
+           "kpn_query_grid", "kpn_mesh_begin", "kpn_mesh_emit", "kpn_render_rays", "kpn_camera_rays", "kpn_render_rays_backward"]
+KPN_ABI_VERSION = 5
 
 c_float_p = C.POINTER(C.c_float)
 c_u8_p = C.POINTER(C.c_uint8)
@@ -68,6 +68,11 @@ class KpnOut(C.Structure):
 
 class KpnRays(C.Structure):
     _fields_ = [("origins", C.c_void_p), ("dirs", C.c_void_p), ("near_far", C.c_void_p), ("n", C.c_longlong), ("mem", C.c_int)]
+
+
+class KpnGrads(C.Structure):
+    _fields_ = [("dW", C.c_void_p * KPN_NUM_LAYERS), ("db", C.c_void_p * KPN_NUM_LAYERS), ("d_ani_al", C.c_void_p),
+                ("d_feat64", C.c_void_p), ("d_feat8", C.c_void_p), ("d_feat_tex", C.c_void_p), ("mem", C.c_int)]
 
 
 class KpnGrid(C.Structure):
@@ -117,6 +122,9 @@ def load() -> C.CDLL:
     lib.kpn_render.restype = C.c_int
     lib.kpn_render_rays.argtypes = [C.c_void_p, C.POINTER(KpnRays), C.POINTER(KpnOpts), C.POINTER(KpnOut), C.c_void_p]
     lib.kpn_render_rays.restype = C.c_int
+    lib.kpn_render_rays_backward.argtypes = [C.c_void_p, C.POINTER(KpnRays), C.POINTER(KpnOpts), C.POINTER(KpnOut),
+                                             C.POINTER(KpnGrads), C.c_void_p]
+    lib.kpn_render_rays_backward.restype = C.c_int
     lib.kpn_camera_rays.argtypes = [C.c_void_p, C.POINTER(KpnTarget), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.kpn_camera_rays.restype = C.c_int
     lib.kpn_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,

@@ -50,6 +50,7 @@ struct kpn_ctx {
   int n_kpt = 0;
   int sp_level = 3;
   float sp_scale = 1.0f, sp_sigma = 0.1f;
+  float ani_al = 0.0f;         // mlp_tex.ani_al as set (the kernels see |ani_al|; its gradient needs the sign)
 
   RawScene* d_raw_scene = nullptr;
   DevScene* d_scene = nullptr;
@@ -62,6 +63,7 @@ struct kpn_ctx {
   TcConsts tcc;                // fp32 constants of the tensor-core engine (kernel parameter)
   bool tc_weights = false;
   int scene_views = 0;
+  int map_hw[3][2] = {};       // (H, W) of the bound scene's feat64, feat8, feat_tex
   int* d_counters = nullptr;   // [MAX_CHUNKS] valid samples per shading batch
   int* d_counters2 = nullptr;  // [MAX_CHUNKS] samples that needed a colour (tensor-core engine)
   int counters_used = 0;
@@ -74,6 +76,9 @@ struct kpn_ctx {
   // records (alpha+sdf, rgb, compositing weight), the fine depths, the colour kernel's latent scratch + work list
   DevBuf ws_rayo, ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
   DevBuf ws_out, ws_in;
+  // kpn_render_rays_backward: staged dL/d outputs, per-list-position gradients (d rad, d sdf | d rgb | a, T), row-major weights,
+  // per-CTA gradient slices and their sum, the three feature-map gradients
+  DevBuf ws_gin, ws_gao, ws_grgb, ws_gat, ws_wr, ws_slices, ws_gred, ws_gmap[3];
   // marching cubes: per-point vertex offsets, per-cell case bytes and face offsets, scan scratch; the state kpn_mesh_begin
   // leaves for kpn_mesh_emit
   DevBuf mc_vofs, mc_cases, mc_tofs, mc_tmp;
@@ -199,7 +204,8 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   c->atlas_fg.release();
   for (DevBuf* b : {&c->ws_rayo, &c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
                     &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in, &c->mc_vofs, &c->mc_cases, &c->mc_tofs,
-                    &c->mc_tmp})
+                    &c->mc_tmp, &c->ws_gin, &c->ws_gao, &c->ws_grgb, &c->ws_gat, &c->ws_wr, &c->ws_slices, &c->ws_gred, &c->ws_gmap[0],
+                    &c->ws_gmap[1], &c->ws_gmap[2]})
     b->release();
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   if (c->h_wd) cudaFreeHost(c->h_wd);
@@ -319,6 +325,7 @@ extern "C" int kpn_set_weights(kpn_ctx* c, const kpn_weights* w) {
     hw.bias[l] = c->wbuf.as<float>() + boff[l];
   }
   hw.ani_al_abs = std::fabs(w->ani_al);
+  c->ani_al = w->ani_al;
   KPN_CUDA(c, cudaMemcpy(c->d_wf32, &hw, sizeof(hw), cudaMemcpyHostToDevice));
   // ---- tensor-core engine: fp16 weight tiles in the interleaved core-matrix layout + fp32 constants
   c->tc_weights = false;
@@ -421,6 +428,7 @@ extern "C" int kpn_set_scene(kpn_ctx* c, const kpn_scene* s, void* stream) {
   for (int m = 0; m < 4; ++m) {
     const MapIn& M = maps[m];
     if (M.H < 1 || M.W < 1) KPN_FAIL(c, KPN_ERR_ARG, "map %d has empty extent", m);
+    if (m < 3) { c->map_hw[m][0] = M.H; c->map_hw[m][1] = M.W; }
     size_t in_bytes = (size_t)V * M.C * M.H * M.W * sizeof(float);
     size_t out_bytes = (size_t)V * M.Cp * M.H * M.W * sizeof(float);
     if (m < 3 && ((s->layout >> m) & 1)) {
@@ -752,6 +760,155 @@ extern "C" int kpn_render_rays(kpn_ctx* c, const kpn_rays* rays, const kpn_opts*
   KPN_CUDA(c, launch_prep_target(nullptr, c->d_target, c->d_scene, st));   // the scene's foreground windows only
   c->launches++;
   return render_rays(c, R, RaySource{false, in.dev<const float>(0), in.dev<const float>(1), in.dev<const float>(2)}, op, out, st);
+}
+
+// The packed gradient vector of the bound weights: every layer's dW (n_out, n_in), its db, then d ani_al.
+static GradLayout grad_layout(const kpn_ctx* c) {
+  int dims[NLAYER][2];
+  expected_dims(c->n_kpt, c->sp_level, dims);
+  GradLayout g;
+  int off = 0;
+  for (int l = 0; l < NLAYER; ++l) { g.wo[l] = off; off += dims[l][0] * dims[l][1]; }
+  for (int l = 0; l < NLAYER; ++l) { g.bo[l] = off; off += dims[l][0]; }
+  g.ani = off;
+  g.total = off + 1;
+  return g;
+}
+
+extern "C" int kpn_render_rays_backward(kpn_ctx* c, const kpn_rays* rays, const kpn_opts* op, const kpn_out* gout, const kpn_grads* gr,
+                                        void* stream) {
+  if (!c || !rays || !op || !gout || !gr || rays->n < 0) return KPN_ERR_ARG;
+  DeviceGuard g(c->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rays->n > 0 && (!rays->origins || !rays->dirs || !rays->near_far)) KPN_FAIL(c, KPN_ERR_ARG, "null ray arrays");
+  if (!mem_ok(rays->mem) || !mem_ok(gout->mem) || !mem_ok(gr->mem)) KPN_FAIL(c, KPN_ERR_ARG, "bad mem kind");
+  for (int l = 0; l < NLAYER; ++l)
+    if (!gr->dW[l] || !gr->db[l]) KPN_FAIL(c, KPN_ERR_ARG, "null gradient of layer %d", l);
+  if (!gr->d_ani_al || !gr->d_feat64 || !gr->d_feat8 || !gr->d_feat_tex) KPN_FAIL(c, KPN_ERR_ARG, "null gradient array");
+  if (!c->have_weights || !c->have_scene) KPN_FAIL(c, KPN_ERR_STATE, "kpn_set_weights and kpn_set_scene must precede kpn_render_rays_backward");
+  if (op->ert_eps > 0.0f)
+    KPN_FAIL(c, KPN_ERR_UNSUPPORTED, "ert_eps > 0: the samples early-ray termination skips have gradients; differentiate with ert_eps = 0");
+  KPN_TRY(wd_check(c, st));
+  const long long R = rays->n;
+  KPN_TRY(check_render(c, op, nullptr, R, gout));
+  const int Sc = op->sample_per_ray_c, Sf = op->fine ? op->sample_per_ray_f : 0;
+  const int Smax = Sc + Sf;
+  const float* a[3] = {rays->origins, rays->dirs, rays->near_far};
+  const Staging in = ray_planes(c, true, rays->mem == KPN_MEM_HOST, R, 3, RAY_W, a);
+  KPN_TRY(stage(c, in, st));
+  const float* gplane[7] = {gout->tex_fg, gout->depth, gout->alpha, gout->tex_fg_fine, gout->depth_fine, gout->alpha_fine, gout->sdf};
+  Staging gin = ray_planes(c, true, gout->mem == KPN_MEM_HOST, R, 7, OUT_W, gplane);
+  gin.buf = &c->ws_gin;
+  KPN_TRY(stage(c, gin, st));
+  const float* gdev[7];
+  for (int i = 0; i < 7; ++i) gdev[i] = gin.dev<const float>(i);
+
+  // gradient accumulators: one slice per CTA of the shading backward, the feature maps, the row-major weights
+  const GradLayout lay = grad_layout(c);
+  const int V = c->scene_views;
+  const int map_c[3] = {64, 8, 8};
+  KPN_CUDA(c, c->ws_wr.reserve((size_t)lay.total * sizeof(float)));
+  KPN_CUDA(c, c->ws_slices.reserve((size_t)c->num_sms * lay.total * sizeof(float)));
+  KPN_CUDA(c, c->ws_gred.reserve((size_t)lay.total * sizeof(float)));
+  KPN_CUDA(c, cudaMemsetAsync(c->ws_slices.p, 0, (size_t)c->num_sms * lay.total * sizeof(float), st));
+  size_t map_bytes[3];
+  for (int m = 0; m < 3; ++m) {
+    map_bytes[m] = (size_t)V * c->map_hw[m][0] * c->map_hw[m][1] * map_c[m] * sizeof(float);
+    KPN_CUDA(c, c->ws_gmap[m].reserve(map_bytes[m]));
+    KPN_CUDA(c, cudaMemsetAsync(c->ws_gmap[m].p, 0, map_bytes[m], st));
+  }
+  KPN_CUDA(c, launch_weights_rowmajor(c->d_wf32, c->ws_wr.as<float>(), lay, st));
+  c->launches++;
+  KPN_CUDA(c, launch_prep_target(nullptr, c->d_target, c->d_scene, st));   // the scene's foreground windows only
+  c->launches++;
+
+  const long long Rc = chunk_rays(R > 0 ? R : 1, Smax);
+  const long long nchunks = (R + Rc - 1) / Rc;
+  if (nchunks * 4 > MAX_CHUNKS) KPN_FAIL(c, KPN_ERR_ARG, "batch too large for one call (%lld chunks)", nchunks);
+  KPN_TRY(reserve_render(c, Rc, Sc, Smax, op->fine != 0, op->fine != 0, false));
+  const size_t n = (size_t)Rc * Smax;
+  KPN_CUDA(c, c->ws_gao.reserve(n * sizeof(float2)));
+  KPN_CUDA(c, c->ws_grgb.reserve(n * 3 * sizeof(float)));
+  KPN_CUDA(c, c->ws_gat.reserve(n * sizeof(float2)));
+  KPN_TRY(begin_counters(c, st));
+  int* seg = c->ws_rayseg.as<int>();
+  int* list = c->ws_list.as<int>();
+  float2* ao = c->ws_ao.as<float2>();
+  float* rgbw = c->ws_rgb.as<float>();
+  float* raynf = c->ws_raynf.as<float>();
+  ShadeGrad sg;
+  sg.d_ao = c->ws_gao.as<float2>(); sg.d_rgb = c->ws_grgb.as<float>(); sg.wr = c->ws_wr.as<float>(); sg.lay = lay;
+  sg.slices = c->ws_slices.as<float>();
+  sg.d_f64 = c->ws_gmap[0].as<float>(); sg.d_f8 = c->ws_gmap[1].as<float>(); sg.d_ftex = c->ws_gmap[2].as<float>();
+  sg.ani_sign = c->ani_al > 0.0f ? 1.0f : (c->ani_al < 0.0f ? -1.0f : 0.0f);
+  // One pass over nr rays x S samples with the fp32 engine (the recorded forward), then its backward: compositing, shading.
+  auto pass = [&](const float* ro, const float* rd, const float* rnf, int r0, int nr, int S, const float* zbuf, int slot, const RayGrad& rg,
+                  float* cw) -> int {
+    SampleSrc src;
+    memset(&src, 0, sizeof(src));
+    src.mode = 0; src.S = S; src.ray_d = rd; src.z = zbuf; src.ray_nf = raynf; src.o = ro;
+    ShadeOut so;
+    memset(&so, 0, sizeof(so));
+    so.ao = ao; so.rgb = rgbw;
+    KPN_CUDA(c, launch_front(c->d_scene, c->d_target, nr, S, zbuf, ro, rd, rnf, raynf, list, 0, c->d_counters + slot, seg, seg + Rc,
+                             ErtSegment{0, 0, nullptr, 0.0f}, st));
+    c->launches++;
+    KPN_TRY(shade_batch(c, src, list, c->d_counters + slot, c->d_counters2 + slot, (long long)nr * S, 0, so, 1, st));
+    if (cw) {
+      KPN_CUDA(c, launch_composite(list, ao, rgbw, seg, seg + Rc, nullptr, nullptr, zbuf, raynf, r0, nr, S, R, nullptr, nullptr, nullptr,
+                                   nullptr, nullptr, cw, st));
+      c->launches++;
+    }
+    KPN_CUDA(c, launch_composite_backward(list, ao, rgbw, seg, seg + Rc, zbuf, raynf, r0, nr, S, R, rg, c->ws_gao.as<float2>(),
+                                          c->ws_grgb.as<float>(), c->ws_gat.as<float2>(), c->num_sms, st));
+    ShadeBatch b;
+    memset(&b, 0, sizeof(b));
+    b.sc = c->d_scene; b.n_views = V; b.n_kpt = c->n_kpt; b.src = src; b.list = list; b.counter = c->d_counters + slot;
+    b.n_max = (long long)nr * S; b.so = so; b.num_sms = c->num_sms; b.st = st; b.wf32 = c->d_wf32; b.launches = &c->launches;
+    KPN_CUDA(c, launch_shade_simt_backward(b, sg));
+    c->launches++;
+    return KPN_OK;
+  };
+  for (long long ch = 0; ch < nchunks; ++ch) {
+    const long long r0 = ch * Rc;
+    const int nr = (int)((R - r0) < Rc ? (R - r0) : Rc);
+    const float* ro = in.dev<const float>(0) + 3 * r0;
+    const float* rd = in.dev<const float>(1) + 3 * r0;
+    const float* rnf = in.dev<const float>(2) + 2 * r0;
+    // coarse pass: its compositing weights drive the resampling (the fine depths carry no gradient, as under the reference's
+    // torch.no_grad), so the fine depths are computed before its list is overwritten
+    KPN_TRY(pass(ro, rd, rnf, (int)r0, nr, Sc, nullptr, (int)(4 * ch), RayGrad{gdev[0], gdev[2], gdev[1], nullptr},
+                 op->fine ? c->ws_cw.as<float>() : nullptr));
+    c->last_total += (unsigned long long)nr * Sc;
+    if (op->fine) {
+      if (op->z_fine_override) {
+        KPN_CUDA(c, cudaMemcpyAsync(c->ws_zfine.p, op->z_fine_override + r0 * Smax, (size_t)nr * Smax * sizeof(float),
+                                    in_kind(gout->mem), st));
+      } else {
+        KPN_CUDA(c, launch_resample(list, c->ws_cw.as<float>(), seg, seg + Rc, nullptr, nullptr, raynf, nr, Sc, Sf, c->ws_zfine.as<float>(),
+                                    nullptr, st));
+        c->launches++;
+      }
+      KPN_TRY(pass(ro, rd, rnf, (int)r0, nr, Smax, c->ws_zfine.as<float>(), (int)(4 * ch + 2),
+                   RayGrad{gdev[3], gdev[5], gdev[4], gdev[6]}, nullptr));
+      c->last_total += (unsigned long long)nr * Smax;
+    }
+  }
+  c->counters_used = (int)(4 * nchunks);
+  KPN_CUDA(c, launch_grad_reduce(c->ws_slices.as<float>(), c->num_sms, lay.total, c->ws_gred.as<float>(), st));
+  c->launches++;
+  const cudaMemcpyKind gkind = gr->mem == KPN_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  const float* red = c->ws_gred.as<float>();
+  for (int l = 0; l < NLAYER; ++l) {
+    const int nw = (l + 1 < NLAYER ? lay.wo[l + 1] : lay.bo[0]) - lay.wo[l];
+    KPN_CUDA(c, cudaMemcpyAsync(gr->dW[l], red + lay.wo[l], (size_t)nw * sizeof(float), gkind, st));
+    KPN_CUDA(c, cudaMemcpyAsync(gr->db[l], red + lay.bo[l], (size_t)((l + 1 < NLAYER ? lay.bo[l + 1] : lay.ani) - lay.bo[l]) * sizeof(float),
+                                gkind, st));
+  }
+  KPN_CUDA(c, cudaMemcpyAsync(gr->d_ani_al, red + lay.ani, sizeof(float), gkind, st));
+  float* dmaps[3] = {gr->d_feat64, gr->d_feat8, gr->d_feat_tex};
+  for (int m = 0; m < 3; ++m) KPN_CUDA(c, cudaMemcpyAsync(dmaps[m], c->ws_gmap[m].p, map_bytes[m], gkind, st));
+  return wd_snapshot(c, st);
 }
 
 extern "C" int kpn_camera_rays(kpn_ctx* c, const kpn_target* tg, float* origins, float* dirs, float* near_far, int mem, void* stream) {

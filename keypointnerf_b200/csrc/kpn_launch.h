@@ -55,6 +55,38 @@ struct ShadeBatch {
   unsigned long long* launches;
 };
 cudaError_t launch_shade_simt(const ShadeBatch& b);
+// ---- backward of the fp32 engine (kpn_grad.cu) ----
+// Where each layer's gradient sits in a packed gradient vector: dW of layer l at wo[l] ((n_out, n_in) row-major, the layout of
+// the folded weight), db at bo[l], d ani_al at ani; `total` floats.  The row-major weight copy (launch_weights_rowmajor) uses
+// the same offsets wo[l].
+struct GradLayout {
+  int wo[NLAYER], bo[NLAYER];
+  int ani, total;
+};
+// The composite backward's inputs (dL/d of one pass' per-ray outputs, planes of `plane` rays at ray r0 + i; nullptr = 0) and
+// per-list-position outputs: d_ao = (d rad, d sdf_raw), d_rgb (3 floats); at = scratch of one float2 per list position.
+struct RayGrad {
+  const float *color, *alpha, *depth, *sdf;
+};
+cudaError_t launch_composite_backward(const int* list, const float2* ao, const float* rgb, const int* start, const int* cnt,
+                                      const float* zbuf, const float* ray_nf, int r0, int nr, int S, long long plane, const RayGrad& g,
+                                      float2* d_ao, float* d_rgb, float2* at, int num_sms, cudaStream_t st);
+// The shading backward of the samples of batch b (b.so.list_base: list position of the batch's first entry): d_ao / d_rgb per
+// list position in, every layer's dW / db / d ani_al added into CTA slice `blockIdx.x` of `slices` (b.num_sms slices of
+// lay.total floats), the feature-map gradients added (atomics) into d_f64 / d_f8 / d_ftex ([V][H][W][C], the atlases' extents).
+struct ShadeGrad {
+  const float2* d_ao;
+  const float* d_rgb;
+  const float* wr;        // row-major copy of every folded weight (launch_weights_rowmajor)
+  GradLayout lay;
+  float* slices;
+  float *d_f64, *d_f8, *d_ftex;
+  float ani_sign;         // sign(ani_al): the layers see |ani_al|
+};
+cudaError_t launch_shade_simt_backward(const ShadeBatch& b, const ShadeGrad& g);
+cudaError_t launch_weights_rowmajor(const DevWeightsF32* w, float* wr, const GradLayout& lay, cudaStream_t st);
+// out[i] = sum over the n slices, in slice order, of slices[s * total + i]
+cudaError_t launch_grad_reduce(const float* slices, int n, int total, float* out, cudaStream_t st);
 cudaError_t launch_shade_tc(const ShadeBatch& b);
 cudaError_t launch_shade_tc_v4(const ShadeBatch& b);   // the 4-view instantiation (kpn_shade_tc_v4.cu)
 size_t tc_pool_bytes(long long n_max);

@@ -23,6 +23,7 @@ import torch.nn as nn
 
 from . import encoders as enc
 from .renderer import RayMarcher
+from .synthetic import layer_table
 
 
 class _WNLinear(nn.Module):
@@ -152,15 +153,15 @@ class KeypointNeRF(nn.Module):
         self.attach_tex_feat(im)
 
     @staticmethod
-    def _encode(module, im, n_down):
-        """avg-pool ``n_down`` times, map [0,1] -> [-1,1], run the encoder channels-last; the outputs' storage is
-        [V][H][W][C], the layout the kernels gather from (no re-layout pass in kpn_set_scene)."""
+    def _encode(module, im, n_down, grad=False):
+        """avg-pool ``n_down`` times, map [0,1] -> [-1,1], run the encoder channels-last (with autograd when ``grad``); the
+        outputs' storage is [V][H][W][C], the layout the kernels gather from (no re-layout pass in kpn_set_scene)."""
         if im.dim() == 5:
             im = im.view(-1, *im.shape[2:])
         x = im.contiguous(memory_format=torch.channels_last)
         for _ in range(n_down):
             x = torch.nn.functional.avg_pool2d(x, 2, stride=2)
-        with torch.no_grad():
+        with torch.set_grad_enabled(grad):
             out = module(2.0 * x - 1.0)
         return [enc.nhwc_view(o) for o in out] if isinstance(out, (list, tuple)) else enc.nhwc_view(out)
 
@@ -503,3 +504,89 @@ class KeypointNeRF(nn.Module):
                             out_device="cuda" if rays_o.is_cuda else "cpu")
         keys = ["tex_fg", "depth", "alpha"] + (["tex_fg_fine", "depth_fine", "alpha_fine", "sdf"] if fine else [])
         return {k: res[k] for k in keys}
+
+    # ---- differentiable explicit rays ---------------------------------------------------------------------------------------
+    def hot_parameters(self):
+        """The parameters the ray-march reads, in the order of ``synthetic.layer_table``: per layer (weight_v, weight_g, bias) of a
+        weight-normed layer or (weight, bias) of a plain one, then ``mlp_tex.ani_al``."""
+        named = dict(self.named_parameters())
+        out = []
+        for name, _, _, wn in layer_table(self.sp_encoder.n_kpt, self.sp_encoder.sp_level):
+            out += [named[name + s] for s in ((".weight_v", ".weight_g", ".bias") if wn else (".weight", ".bias"))]
+        return out + [self.mlp_tex.ani_al]
+
+    @staticmethod
+    def render_rays_grad(net, img_in, cam_in, rays_o, rays_d, near_far, sp_data={}, **config):
+        """``render_rays`` with outputs that carry a ``grad_fn``: ``loss.backward()`` reaches every hot-path parameter
+        (``hot_parameters``) and the feature maps ``feat_geo[0]``, ``feat_geo[1]``, ``feat_tex`` (the gradients are computed by
+        ``kpn_render_rays_backward``: fp32 CUDA cores, the reference's autograd semantics of the eval branch).  Same keys,
+        refusals and outputs as ``render_rays``; the forward runs on ``net.engine``.  Without ``feat_geo`` / ``feat_tex`` the
+        encoders run here with autograd (and without the feature cache), so that the gradient reaches them too.  The fine
+        pass' depths, the source images, cameras, keypoints, bounds, rays and masks get no gradient."""
+        config = dict(config)
+        feat_geo = config.pop("feat_geo", None)
+        feat_tex = config.pop("feat_tex", None)
+        KeypointNeRF._check_config(config)
+        if config.get("ert_eps", 0.0) > 0.0:
+            raise NotImplementedError("ert_eps > 0: the samples early-ray termination skips have gradients")
+        if feat_geo is None:
+            if net.geo_encoder is None:
+                raise RuntimeError("this model was built without geo_args: pass feat_geo explicitly")
+            feat_geo = KeypointNeRF._encode(net.geo_encoder, img_in, net.ds_geo, grad=True)
+        if feat_tex is None:
+            if net.tex_encoder is None:
+                raise RuntimeError("this model was built without tex_args: pass feat_tex explicitly")
+            feat_tex = KeypointNeRF._encode(net.tex_encoder, img_in, net.ds_tex, grad=True)
+        fine = config.get("fine", False)
+        keys = ["tex_fg", "depth", "alpha"] + (["tex_fg_fine", "depth_fine", "alpha_fine", "sdf"] if fine else [])
+        opts = dict(S_c=config.get("sample_per_ray_c", 64), S_f=config.get("sample_per_ray_f", 64), fine=fine)
+        fg = config.get("src_foreground_mask")
+        bind = lambda: net._bind_scene(cam_in, feat_geo, feat_tex, sp_data, img_in, fg, config["bounds"])
+        outs = _RenderRays.apply(net, bind, (rays_o, rays_d, near_far), opts, keys, feat_geo[0], feat_geo[1], feat_tex,
+                                 *net.hot_parameters())
+        return dict(zip(keys, outs))
+
+
+def param_grads(net, g, params):
+    """The gradients of ``hot_parameters`` (``params``, in that order) from ``RayMarcher.render_rays_backward``'s ``g``: the folded
+    weight ``W = g v / ||v||`` of a weight-normed layer maps per row to ``dg = sum_k dW v / ||v||``,
+    ``dv = (g / ||v||) (dW - (dW . v^) v^)``."""
+    out, i = [], 0
+    for l, (_, _, _, wn) in enumerate(layer_table(net.sp_encoder.n_kpt, net.sp_encoder.sp_level)):
+        dW, db = g["dW"][l], g["db"][l]
+        if wn:
+            v, gw = params[i], params[i + 1]
+            nrm = v.norm(dim=1, keepdim=True)
+            vh = v / nrm
+            proj = (dW * vh).sum(1, keepdim=True)
+            out += [(gw / nrm) * (dW - proj * vh), proj.to(gw.dtype), db]
+            i += 3
+        else:
+            out += [dW, db]
+            i += 2
+    out.append(g["d_ani_al"].reshape(params[i].shape))
+    return out
+
+
+class _RenderRays(torch.autograd.Function):
+    """Forward: ``RayMarcher.render_rays`` on ``net.engine``; backward: ``RayMarcher.render_rays_backward`` at the fine depths the
+    forward resampled (its outputs' own), then ``param_grads``.  First order only."""
+
+    @staticmethod
+    def forward(ctx, net, bind, rays, opts, keys, feat64, feat8, feat_tex, *params):
+        m = bind()
+        res = m.render_rays(*rays, **opts, engine=net.engine, debug=opts["fine"],
+                            out_device="cuda" if rays[0].is_cuda else "cpu")
+        ctx.net, ctx.bind, ctx.rays, ctx.opts, ctx.keys = net, bind, rays, opts, keys
+        ctx.z_fine = res.get("z_fine")
+        ctx.save_for_backward(*params)
+        return tuple(res[k] for k in keys)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, *grads):
+        m = ctx.bind()
+        g = m.render_rays_backward(*ctx.rays, {k: v for k, v in zip(ctx.keys, grads) if v is not None}, **ctx.opts,
+                                   z_fine_override=ctx.z_fine)
+        maps = [g["d_feat64"], g["d_feat8"], g["d_feat_tex"]]
+        return (None, None, None, None, None, *maps, *param_grads(ctx.net, g, ctx.saved_tensors))

@@ -43,6 +43,8 @@ class RayMarcher:
                              "(a CUDA device is required; there is no CPU fallback)")
         self._keep = []       # tensors that must outlive the asynchronous calls of the current scene
         self.n_views = 0
+        self.n_kpt, self.sp_level = 0, 3                                  # of the weights set last
+        self.map_shapes = [(0, 64, 1, 1), (0, 8, 1, 1), (0, 8, 1, 1)]      # (V, C, H, W) of the bound scene's gathered maps
 
     def close(self):
         if getattr(self, "ctx", None) is not None and self.ctx.value:
@@ -86,7 +88,7 @@ class RayMarcher:
         w.ani_al = float(np.asarray(host(state["mlp_tex.ani_al"])).reshape(-1)[0])
         w.n_kpt, w.sp_level, w.sp_scale, w.sp_sigma = int(n_kpt), int(sp_level), float(sp_scale), float(sp_sigma)
         L.check(self.lib, self.ctx, self.lib.kpn_set_weights(self.ctx, C.byref(w)), "kpn_set_weights")
-        self.n_kpt = int(n_kpt)
+        self.n_kpt, self.sp_level = int(n_kpt), int(sp_level)
 
     # ---- scene ---------------------------------------------------------------------------------
     def set_scene(self, *, KRT, extrin, kpt3d, bounds, feat64, feat8, feat_tex, img, fg, width, height,
@@ -136,6 +138,7 @@ class RayMarcher:
         L.check(self.lib, self.ctx, self.lib.kpn_set_scene(self.ctx, C.byref(s), self._stream()), "kpn_set_scene")
         self._keep = keep
         self.n_views = V
+        self.map_shapes = [tuple(feat64.shape), tuple(feat8.shape), tuple(feat_tex.shape)]
 
     # ---- render --------------------------------------------------------------------------------
     def reserve(self, max_rays: int, max_samples: int):
@@ -243,6 +246,60 @@ class RayMarcher:
         call = lambda op, out: self.lib.kpn_render_rays(self.ctx, C.byref(rays), op, out, self._stream())
         return self._march(call, "kpn_render_rays", (n,), out_device, S_c, S_f, fine, engine, z_fine_override, debug, ert_eps,
                            [o, d, nf])
+
+    _GRAD_KEYS = ("tex_fg", "depth", "alpha", "tex_fg_fine", "depth_fine", "alpha_fine", "sdf")
+
+    def render_rays_backward(self, origins, dirs, near_far, grad_out: dict, *, S_c, S_f=0, fine=False, ert_eps=0.0,
+                             z_fine_override=None) -> dict:
+        """The backward of ``render_rays`` (``kpn_render_rays_backward``): ``grad_out`` maps output names of ``render_rays``
+        (``tex_fg`` (3,n), ``depth``, ``alpha`` (n,), with ``fine`` also ``tex_fg_fine``, ``depth_fine``, ``alpha_fine``,
+        ``sdf``) to dL/d that output; a missing key is zero.  Returns device tensors on this context's device: ``dW`` and ``db``
+        (lists over the layers of ``synthetic.layer_table``, ``dW[l]`` (n_out, n_in) of the folded weight ``g v / ||v||``),
+        ``d_ani_al`` (scalar) and ``d_feat64``, ``d_feat8``, ``d_feat_tex`` shaped (V, C, H, W) like the bound maps, stored
+        channels-last.  The forward is recomputed with the fp32 engine; the fine depths are constants."""
+        dev = torch.device("cuda", self.device)
+        o = _f32c(origins).reshape(-1, 3).to(dev).contiguous()
+        d, nf = _f32c(dirs).reshape(-1, 3).to(dev).contiguous(), _f32c(near_far).reshape(-1, 2).to(dev).contiguous()
+        n = o.shape[0]
+        if d.shape[0] != n or nf.shape[0] != n:
+            raise ValueError(f"render_rays_backward: {n} origins, {d.shape[0]} directions, {nf.shape[0]} near/far pairs")
+        rays = L.KpnRays()
+        rays.origins, rays.dirs, rays.near_far, rays.n, rays.mem = o.data_ptr(), d.data_ptr(), nf.data_ptr(), n, L.KPN_MEM_DEVICE
+        op = L.KpnOpts()
+        op.sample_per_ray_c, op.sample_per_ray_f, op.fine = int(S_c), int(S_f), int(bool(fine))
+        op.ert_eps, op.engine = float(ert_eps), 1
+        keep = [o, d, nf]
+        if z_fine_override is not None:
+            zo = _f32c(z_fine_override).to(dev).contiguous()
+            assert zo.numel() == n * (S_c + S_f)
+            op.z_fine_override = zo.data_ptr()
+            keep.append(zo)
+        gout = L.KpnOut()
+        for k, v in grad_out.items():
+            if k not in self._GRAD_KEYS:
+                raise ValueError(f"render_rays_backward: no output {k!r}")
+            if v is None:
+                continue
+            g = _f32c(v).to(dev).contiguous()
+            if g.numel() != (3 * n if k.startswith("tex_fg") else n):
+                raise ValueError(f"render_rays_backward: dL/d{k} has {g.numel()} values for {n} rays")
+            setattr(gout, k, g.data_ptr())
+            keep.append(g)
+        gout.mem = L.KPN_MEM_DEVICE
+        gr = L.KpnGrads()
+        dW, db = [], []
+        for i, (_, n_out, n_in, _) in enumerate(layer_table(self.n_kpt, self.sp_level)):
+            dW.append(torch.empty(n_out, n_in, dtype=torch.float32, device=dev))
+            db.append(torch.empty(n_out, dtype=torch.float32, device=dev))
+            gr.dW[i], gr.db[i] = dW[-1].data_ptr(), db[-1].data_ptr()
+        d_ani = torch.empty((), dtype=torch.float32, device=dev)
+        maps = [torch.empty(s, dtype=torch.float32, device=dev, memory_format=torch.channels_last) for s in self.map_shapes]
+        gr.d_ani_al, gr.d_feat64, gr.d_feat8, gr.d_feat_tex = d_ani.data_ptr(), *(m.data_ptr() for m in maps)
+        gr.mem = L.KPN_MEM_DEVICE
+        L.check(self.lib, self.ctx, self.lib.kpn_render_rays_backward(self.ctx, C.byref(rays), C.byref(op), C.byref(gout), C.byref(gr),
+                                                                       self._stream()), "kpn_render_rays_backward")
+        self._keep_call = keep
+        return {"dW": dW, "db": db, "d_ani_al": d_ani, "d_feat64": maps[0], "d_feat8": maps[1], "d_feat_tex": maps[2]}
 
     def query(self, pts: torch.Tensor, view: torch.Tensor, engine: int = 0):
         """``KeypointNeRF.query`` for explicit points: returns out (n,5)=[sdf_raw, rad, r, g, b], valid (n,) bool."""
