@@ -77,8 +77,9 @@ struct kpn_ctx {
   DevBuf ws_rayo, ws_rayd, ws_raynf, ws_rayseg, ws_list, ws_ao, ws_rgb, ws_cw, ws_zfine, ws_lat, ws_list2, ws_ert, ws_contrib, ws_pool;
   DevBuf ws_out, ws_in;
   // kpn_render_rays_backward: staged dL/d outputs, per-list-position gradients (d rad, d sdf | d rgb | a, T), row-major weights,
-  // per-CTA gradient slices and their sum, the three feature-map gradients
-  DevBuf ws_gin, ws_gao, ws_grgb, ws_gat, ws_wr, ws_slices, ws_gred, ws_gmap[3];
+  // per-CTA gradient slices and their sum, the three feature-map gradients, the front's work list and ray starts before they are
+  // put in ray order and the scan scratch that does it
+  DevBuf ws_gin, ws_gao, ws_grgb, ws_gat, ws_wr, ws_slices, ws_gred, ws_gmap[3], ws_glist, ws_gscan;
   // marching cubes: per-point vertex offsets, per-cell case bytes and face offsets, scan scratch; the state kpn_mesh_begin
   // leaves for kpn_mesh_emit
   DevBuf mc_vofs, mc_cases, mc_tofs, mc_tmp;
@@ -205,7 +206,7 @@ extern "C" void kpn_destroy(kpn_ctx* c) {
   for (DevBuf* b : {&c->ws_rayo, &c->ws_rayd, &c->ws_raynf, &c->ws_rayseg, &c->ws_list, &c->ws_ao, &c->ws_rgb, &c->ws_cw, &c->ws_zfine, &c->ws_lat,
                     &c->ws_list2, &c->ws_ert, &c->ws_contrib, &c->ws_pool, &c->ws_out, &c->ws_in, &c->mc_vofs, &c->mc_cases, &c->mc_tofs,
                     &c->mc_tmp, &c->ws_gin, &c->ws_gao, &c->ws_grgb, &c->ws_gat, &c->ws_wr, &c->ws_slices, &c->ws_gred, &c->ws_gmap[0],
-                    &c->ws_gmap[1], &c->ws_gmap[2]})
+                    &c->ws_gmap[1], &c->ws_gmap[2], &c->ws_glist, &c->ws_gscan})
     b->release();
   for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
   if (c->h_wd) cudaFreeHost(c->h_wd);
@@ -830,6 +831,9 @@ extern "C" int kpn_render_rays_backward(kpn_ctx* c, const kpn_rays* rays, const 
   KPN_CUDA(c, c->ws_gao.reserve(n * sizeof(float2)));
   KPN_CUDA(c, c->ws_grgb.reserve(n * 3 * sizeof(float)));
   KPN_CUDA(c, c->ws_gat.reserve(n * sizeof(float2)));
+  KPN_CUDA(c, c->ws_glist.reserve((n + (size_t)Rc) * sizeof(int)));
+  const size_t scan_bytes = canonical_list_temp_bytes((int)Rc);
+  KPN_CUDA(c, c->ws_gscan.reserve(scan_bytes));
   KPN_TRY(begin_counters(c, st));
   int* seg = c->ws_rayseg.as<int>();
   int* list = c->ws_list.as<int>();
@@ -841,7 +845,12 @@ extern "C" int kpn_render_rays_backward(kpn_ctx* c, const kpn_rays* rays, const 
   sg.slices = c->ws_slices.as<float>();
   sg.d_f64 = c->ws_gmap[0].as<float>(); sg.d_f8 = c->ws_gmap[1].as<float>(); sg.d_ftex = c->ws_gmap[2].as<float>();
   sg.ani_sign = c->ani_al > 0.0f ? 1.0f : (c->ani_al < 0.0f ? -1.0f : 0.0f);
-  // One pass over nr rays x S samples with the fp32 engine (the recorded forward), then its backward: compositing, shading.
+  // One pass over nr rays x S samples with the fp32 engine (the recorded forward), then its backward: compositing, shading.  The
+  // front's work list is put in ray order first (launch_canonical_list): which samples share a tile of the shading backward, and
+  // so the summation order of dW, db and d ani_al, then depends on the rays alone and not on the order in which the front's
+  // blocks won their atomics.
+  int* raw_list = c->ws_glist.as<int>();
+  int* raw_start = raw_list + n;
   auto pass = [&](const float* ro, const float* rd, const float* rnf, int r0, int nr, int S, const float* zbuf, int slot, const RayGrad& rg,
                   float* cw) -> int {
     SampleSrc src;
@@ -850,9 +859,10 @@ extern "C" int kpn_render_rays_backward(kpn_ctx* c, const kpn_rays* rays, const 
     ShadeOut so;
     memset(&so, 0, sizeof(so));
     so.ao = ao; so.rgb = rgbw;
-    KPN_CUDA(c, launch_front(c->d_scene, c->d_target, nr, S, zbuf, ro, rd, rnf, raynf, list, 0, c->d_counters + slot, seg, seg + Rc,
-                             ErtSegment{0, 0, nullptr, 0.0f}, st));
-    c->launches++;
+    KPN_CUDA(c, launch_front(c->d_scene, c->d_target, nr, S, zbuf, ro, rd, rnf, raynf, raw_list, 0, c->d_counters + slot, raw_start,
+                             seg + Rc, ErtSegment{0, 0, nullptr, 0.0f}, st));
+    KPN_CUDA(c, launch_canonical_list(raw_list, raw_start, seg + Rc, nr, list, seg, c->ws_gscan.p, scan_bytes, c->num_sms, st));
+    c->launches += 3;
     KPN_TRY(shade_batch(c, src, list, c->d_counters + slot, c->d_counters2 + slot, (long long)nr * S, 0, so, 1, st));
     if (cw) {
       KPN_CUDA(c, launch_composite(list, ao, rgbw, seg, seg + Rc, nullptr, nullptr, zbuf, raynf, r0, nr, S, R, nullptr, nullptr, nullptr,

@@ -8,6 +8,10 @@
 //                        then backpropagates colour head -> density head -> view pooling -> per-view geometry MLP (each view's
 //                        activations rebuilt in turn); dW / db into the CTA's own slice, feature-map taps scattered with atomics
 //   grad_reduce          the CTA slices summed in CTA order (deterministic)
+//   canonical_list       the front kernel's work list rewritten in ray order, so that the tiles above (and with them the
+//                        summation order of dW, db and d ani_al) depend on the rays alone
+#include <cub/device/device_scan.cuh>
+
 #include "kpn_launch.h"
 #include "kpn_simt.cuh"
 
@@ -640,8 +644,22 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
       for (int v = 0; v < V; ++v) {
         const float f = F[(v * GTS + r) * 36 + c], dlt = f - mean, w = Om[v * GTS + r];
         dF[(v * GTS + r) * 36 + c] += w * (dmean + 2.0f * dlt * dvar);
-        atomicAdd(dOm + v * GTS + r, dmean * f + dvar * dlt * dlt);
       }
+      float* mdv = sm + SM::GA2 + r * 108;   // mean, dmean, dvar of (r, c) for the blend-weight gradient below
+      mdv[c] = mean; mdv[35 + c] = dmean; mdv[70 + c] = dvar;
+    }
+    __syncthreads();
+    // d Om_v += sum_c dmean f + dvar (f - mean)^2, one thread per (view, row) summing the channels in order (reproducible)
+    for (int idx = t; idx < V * GTS; idx += GNT) {
+      const int r = idx % GTS;
+      const float* f = F + idx * 36;
+      const float* mdv = sm + SM::GA2 + r * 108;
+      float s = 0.0f;
+      for (int c = 0; c < 35; ++c) {
+        const float dlt = f[c] - mdv[c];
+        s += mdv[35 + c] * f[c] + mdv[70 + c] * dlt * dlt;
+      }
+      dOm[idx] += s;
     }
     __syncthreads();
     // ---- 9. ray encoder backward per view; d tex -> feature map; d latent
@@ -702,7 +720,10 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
         for (int v = 0; v < V; ++v) s += (du - dOm[v * GTS + t]) * w[v];
         da += s * inv * inv * dwda[u];
       }
-      atomicAdd(sMisc, da);
+      // the tile's sum over its rows by a fixed butterfly (warp 0 holds the GTS = 32 rows), added by one thread (reproducible)
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) da += __shfl_xor_sync(0xffffffffu, da, d);
+      if (t == 0) sMisc[0] += da;
     }
     __syncthreads();
     // ---- 11. latent backward (ibr_compress_gfeat): dPool += Wc^T dLat
@@ -783,6 +804,39 @@ __global__ void grad_reduce_kernel(const float* __restrict__ slices, int n, int 
     for (int b = 0; b < n; ++b) s += slices[(size_t)b * total + i];
     out[i] = s;
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// canonical work list
+// ------------------------------------------------------------------------------------------------
+// The front kernel's blocks reserve their ranges of the work list with an atomicAdd each, so the order of the rays in its list
+// changes from call to call.  Rewritten with every ray's entries (in sample order, as the front wrote them) at the exclusive
+// scan of the counts in ray order, the list is a function of the rays alone.  One warp per ray.
+__global__ void canonical_list_kernel(const int* __restrict__ list_in, const int* __restrict__ start_in, const int* __restrict__ cnt,
+                                      const int* __restrict__ start_out, int nr, int* __restrict__ list_out) {
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  for (int i = blockIdx.x * wpb + (threadIdx.x >> 5); i < nr; i += gridDim.x * wpb) {
+    const int a = start_in[i], b = start_out[i], n = cnt[i];
+    for (int j = lane; j < n; j += 32) list_out[b + j] = list_in[a + j];
+  }
+}
+
+size_t canonical_list_temp_bytes(int nr) {
+  size_t bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const int*)nullptr, (int*)nullptr, nr);
+  return bytes;
+}
+
+cudaError_t launch_canonical_list(const int* list_in, const int* start_in, const int* cnt, int nr, int* list_out, int* start_out,
+                                  void* scan_tmp, size_t scan_bytes, int num_sms, cudaStream_t st) {
+  if (nr < 1) return cudaSuccess;
+  cudaError_t e = cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, cnt, start_out, nr, st);   // deterministic
+  if (e != cudaSuccess) return e;
+  long long blocks = ((long long)nr * 32 + 255) / 256;
+  if (blocks > (long long)num_sms * 16) blocks = (long long)num_sms * 16;
+  canonical_list_kernel<<<(unsigned)blocks, 256, 0, st>>>(list_in, start_in, cnt, start_out, nr, list_out);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_composite_backward(const int* list, const float2* ao, const float* rgb, const int* start, const int* cnt,

@@ -84,6 +84,11 @@ struct ShadeGrad {
   float ani_sign;         // sign(ani_al): the layers see |ani_al|
 };
 cudaError_t launch_shade_simt_backward(const ShadeBatch& b, const ShadeGrad& g);
+// The work list of one pass rewritten in ray order: start_out = the exclusive scan of cnt (nr rays), ray i's cnt[i] entries copied
+// from list_in[start_in[i] ..] to list_out[start_out[i] ..].  scan_tmp holds canonical_list_temp_bytes(nr) bytes.
+size_t canonical_list_temp_bytes(int nr);
+cudaError_t launch_canonical_list(const int* list_in, const int* start_in, const int* cnt, int nr, int* list_out, int* start_out,
+                                  void* scan_tmp, size_t scan_bytes, int num_sms, cudaStream_t st);
 cudaError_t launch_weights_rowmajor(const DevWeightsF32* w, float* wr, const GradLayout& lay, cudaStream_t st);
 // out[i] = sum over the n slices, in slice order, of slices[s * total + i]
 cudaError_t launch_grad_reduce(const float* slices, int n, int total, float* out, cudaStream_t st);

@@ -17,116 +17,21 @@ from keypointnerf_b200 import synthetic as syn
 from keypointnerf_b200.model import KeypointNeRF, param_grads
 from keypointnerf_b200.renderer import RayMarcher
 from keypointnerf_b200.testing import build_model, scene_tensors
-from oracle import kpnerf_oracle as O  # checker only
 from tests import grad_oracle as GO
-from tests import rays_oracle as RO
 
 pytestmark = pytest.mark.gpu
 
-DEV = "cuda:0"
+DEV = GO.DEV
 MAPS = GO.MAPS
-FINE_KEYS = ["tex_fg", "depth", "alpha", "tex_fg_fine", "depth_fine", "alpha_fine", "sdf"]
-GATE = 1e-4
+GATE = GO.GATE
 SP3 = {"sp_level": 3, "scale": 1.0, "sigma": 0.1}
-
-
-def _rays(target, n):
-    """The rays of an n x n lattice of the target camera (fp32, as the library marches them)."""
-    pix = O.pixel_lattice(n, n, 1, 0, 0)
-    o, d, n_r, f_r = O.ray_setup(pix, target["K"], target["RT"], float(target["znear"]), float(target["zfar"]))
-    return o.expand(d.shape[0], 3).contiguous(), d.contiguous(), torch.cat([n_r, f_r], -1).contiguous()
-
-
-def _loss_weights(n, seed=11):
-    gen = torch.Generator().manual_seed(seed)
-    return {k: torch.randn((3, n) if k.startswith("tex_fg") else (n,), generator=gen) for k in FINE_KEYS}
-
-
-def _setup(n_views, n_kpt, sp_level, n, S_c, S_f, src_size=64):
-    scene = syn.make_scene(src_size=src_size, n_views=n_views, n_kpt=n_kpt, fg_mode="hull")
-    target = syn.make_target(size=n, zoom=2.0)
-    sp = {"sp_level": sp_level, "scale": 1.0, "sigma": 0.1}
-    weights = syn.make_weights(n_kpt, sp_level=sp_level)
-    net = build_model(weights, n_kpt, DEV, sp_args=sp)
-    net.engine = 1
-    a = scene_tensors(scene, target, DEV)
-    o, d, nf = _rays(target, n)
-    return scene, weights, sp, net, a, (o, d, nf)
-
-
-def _oracle_grads(scene, weights, sp, rays, S_c, S_f, z_fine, G):
-    """fp64 autograd of the oracle: (d weights by state_dict name, d maps by scene key, outputs)."""
-    return GO.oracle_grads(scene, weights, sp, rays, S_c, S_f, z_fine, G)
-
-
-def _gpu_grads(net, a, rays, S_c, S_f, G):
-    feats = [a["feat_geo"][0].clone().requires_grad_(), a["feat_geo"][1].clone().requires_grad_(), a["feat_tex"].clone().requires_grad_()]
-    net.zero_grad(set_to_none=True)
-    cfg = dict(sample_per_ray_c=S_c, sample_per_ray_f=S_f, fine=True, uniform=True, src_foreground_mask=a["fg"], bounds=a["bounds"],
-               feat_geo=feats[:2], feat_tex=feats[2])
-    out = net.render_rays_grad(net, a["img"], a["cam"], *(t.to(DEV) for t in rays), sp_data=a["sp_data"], **cfg)
-    loss = sum((out[k] * G[k].to(DEV)).sum() for k in G)
-    loss.backward()
-    torch.cuda.synchronize()
-    return dict(net.named_parameters()), dict(zip(MAPS, (f.grad for f in feats))), out
-
-
-def _compare(got, ref, name, rep):
-    got, ref = got.detach().double().cpu().reshape(-1), ref.detach().double().cpu().reshape(-1)
-    nrm = float(ref.norm())
-    rel = float((got - ref).norm()) / nrm if nrm > 0 else float(got.norm())
-    mx = float((got - ref).abs().max()) / max(float(ref.abs().max()), 1e-30) if nrm > 0 else float(got.abs().max())
-    ok = rel <= GATE and mx <= GATE
-    if not ok or rel > GATE / 10:
-        rep.append(f"{name}: rel L2 {rel:.2e}, max {mx:.2e}")
-    return ok
-
-
-def _check_ani_al(g, ref, n_views, rep):
-    """ani_al reaches the loss only through the blend weights Om_v = w_v / (sum w + 1e-8), w_v = ex_v - min ex.  Where a view's ex
-    nearly ties with the minimum, its w_v is a difference of nearly equal exponentials that the fp32 forward resolves only to
-    ~1e-7 / w_v relative (the backward rebuilds w_v with expm1, but the forward's Om_v and dot products carry that error), and dOm_v
-    carries it into d ani_al: this one scalar is gated at 1e-3 relative.  With two views, w of one view is 0 and the other's
-    Om = w / (w + 1e-8) depends on ani_al only through the 1e-8 term: its gradient is pure 1 / w^2 conditioning, and only its sign
-    and size (within 2x) are checked."""
-    got, want = float(g), float(ref)
-    ok = abs(got - want) <= 1e-3 * abs(want) if n_views != 2 else (got * want > 0 and 0.5 < got / want < 2.0)
-    if not ok or abs(got - want) > GATE * abs(want):
-        rep.append(f"mlp_tex.ani_al: {got:.6e} vs {want:.6e}")
-    return ok
+_setup = GO.setup
+_loss_weights = GO.loss_weights
 
 
 def _check_against_oracle(n_views, n_kpt, sp_level, n, S_c, S_f):
-    scene, weights, sp, net, a, rays = _setup(n_views, n_kpt, sp_level, n, S_c, S_f)
-    m = net._bind_scene(a["cam"], a["feat_geo"], a["feat_tex"], a["sp_data"], a["img"], a["fg"], a["bounds"])
-    fwd = m.render_rays(*(t.to(DEV) for t in rays), S_c=S_c, S_f=S_f, fine=True, engine=1, debug=True)
-    z_fine = fwd["z_fine"].cpu()
-    G = _loss_weights(rays[0].shape[0])
-    params, dmaps, out = _gpu_grads(net, a, rays, S_c, S_f, G)
-    w_ref, m_ref, _ = _oracle_grads(scene, weights, sp, rays, S_c, S_f, z_fine, G)
-    assert float(fwd["alpha_fine"].max()) > 0.05, "empty frame"
-    rep, good = [], True
-    for k, ref in w_ref.items():
-        g = params[k].grad
-        assert g is not None and bool(torch.isfinite(g).all()), k
-        if k == "mlp_tex.out_layer.4.bias":
-            # the softmax over the views is shift invariant: the exact gradient of the last colour layer's bias is 0 (fp64 leaves
-            # ~1e-17), so its error is gated against the scale of the same layer's weight gradient
-            scale = float(w_ref["mlp_tex.out_layer.4.weight"].abs().max())
-            ok = float(g.abs().max()) <= GATE * scale and float(ref.abs().max()) <= 1e-9 * scale
-            if not ok:
-                rep.append(f"{k}: |got| {float(g.abs().max()):.2e}, |ref| {float(ref.abs().max()):.2e}, scale {scale:.2e}")
-            good &= ok
-            continue
-        if k == "mlp_tex.ani_al":
-            good &= _check_ani_al(g, ref, n_views, rep)
-            continue
-        good &= _compare(g, ref.reshape(g.shape), k, rep)
-    for k in MAPS:
-        good &= _compare(dmaps[k], m_ref[k], k, rep)
-    print(f"{n_views} views, {n_kpt} kpt, sp_level {sp_level}, {n}x{n} rays, S {S_c}+{S_f}: " + ("; ".join(rep) or "all within 1e-5"))
-    assert good, rep
-    m.check_health()
+    scene, weights, sp, net, a, rays = _setup(n_views, n_kpt, sp_level, n)
+    GO.check_against_oracle(net, a, scene, weights, sp, rays, S_c, S_f, label=f"{n_kpt} kpt, sp_level {sp_level}: ")
 
 
 @pytest.mark.parametrize("n_views", [1, 2, 3, 4])
@@ -151,7 +56,7 @@ def test_training_patch_against_oracle():
 
 @pytest.mark.parametrize("engine", [0, 1])
 def test_outputs_equal_render_rays(engine):
-    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 12, 16, 16)
+    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 12)
     net.engine = engine
     cfg = dict(sample_per_ray_c=16, sample_per_ray_f=16, fine=True, uniform=True, src_foreground_mask=a["fg"], bounds=a["bounds"],
                feat_geo=a["feat_geo"], feat_tex=a["feat_tex"])
@@ -172,7 +77,7 @@ def _all_grads(g):
 
 
 def test_no_valid_sample_and_empty_batch_give_zero_gradients():
-    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 8, 16, 16)
+    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 8)
     m = net._bind_scene(a["cam"], a["feat_geo"], a["feat_tex"], a["sp_data"], a["img"], a["fg"], a["bounds"])
     o, d, nf = (t.to(DEV) for t in rays)
     away = -d   # rays that leave the scene: no valid sample
@@ -188,7 +93,7 @@ def test_no_valid_sample_and_empty_batch_give_zero_gradients():
 
 
 def test_refusals():
-    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 8, 16, 16)
+    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 8)
     r = [t.to(DEV) for t in rays]
     cfg = dict(sample_per_ray_c=16, sample_per_ray_f=16, fine=True, uniform=True, src_foreground_mask=a["fg"], bounds=a["bounds"],
                feat_geo=a["feat_geo"], feat_tex=a["feat_tex"])
@@ -220,7 +125,7 @@ def test_refusals():
 def test_backward_reaches_the_encoders():
     """Without feat_geo / feat_tex the encoders run with autograd: loss.backward() leaves finite, non-zero gradients on the hot-path
     parameters and on the encoders' parameters."""
-    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 12, 16, 16, src_size=256)   # the encoders downsample 64x
+    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 12, src_size=256)   # the encoders downsample 64x
     assert net.geo_encoder is not None and net.tex_encoder is not None
     cfg = dict(sample_per_ray_c=16, sample_per_ray_f=16, fine=True, uniform=True, src_foreground_mask=a["fg"], bounds=a["bounds"])
     for seed in range(26, 46):   # the first weights whose density is positive somewhere on the encoders' (random) features
@@ -243,7 +148,7 @@ def test_backward_reaches_the_encoders():
 
 def test_adam_fits_a_render_of_other_weights():
     """20 Adam steps on the hot-path parameters lower the L1 loss against a render of different weights."""
-    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 16, 32, 32)
+    scene, weights, sp, net, a, rays = _setup(3, 18, 3, 16)
     r = [t.to(DEV) for t in rays]
     cfg = dict(sample_per_ray_c=32, sample_per_ray_f=32, fine=True, uniform=True, src_foreground_mask=a["fg"], bounds=a["bounds"],
                feat_geo=a["feat_geo"], feat_tex=a["feat_tex"])
@@ -291,7 +196,7 @@ def test_gradients_match_reference_goldens(name):
         if k == "mlp_tex.out_layer.4.bias":   # exact gradient 0 (the softmax over views is shift invariant)
             ok = float(v.abs().max()) <= GATE * scale
         else:
-            gate = 1e-3 if k == "mlp_tex.ani_al" else GATE   # see _check_ani_al
+            gate = 1e-3 if k == "mlp_tex.ani_al" else GATE   # see GO.check_ani_al
             x = exact[k].reshape(v.shape)
             e, ex, e64 = GO.rel_errors(v, g["g/" + k]), GO.rel_errors(v, x), GO.rel_errors(x, g["g/" + k])
             ok = all(x <= max(gate, 2.0 * y) for x, y in zip(ex, e64))
