@@ -715,8 +715,12 @@ geo_front_kernel(const DevScene* __restrict__ scp, int nk, const uint8_t* __rest
 
 
 // =====================================================================================================================
-// colour head.  Warpgroup tile = 128 rows (4 row warps x spw(NV) samples x NV views: 40 samples with 3 views, 32 with 4; each
-// stage runs as two 64-row MMAs whose accumulators are staged in shared memory (D) for the row threads, which do the cross-view work of the reference.
+// colour head.  Warpgroup tile = 128 rows (4 row warps x spw(NV) samples x NV views: 40 samples with 3 views, 32 with 4).  Each
+// stage issues its two 64-row MMAs back to back and retires them with one wait.  BASE0 and VIS1A, whose epilogues are elementwise,
+// write the next stage's activation tile straight from their fragments; the other stages stage their accumulators in shared
+// memory (D) for the row threads, which do the cross-view work of the reference.  Two tiles are in flight per warpgroup: while a
+// tile runs its stages, the row threads fetch the next tile's inputs (work-list entry beside RE1, sample and latent beside BASE0,
+// projection and ray difference beside BASE1, img / feat_tex taps beside OUT0), so a tile starts on no global load.
 // =====================================================================================================================
 constexpr int CWG = 3;                                   // warpgroups per CTA (168 registers per thread)
 constexpr int CDS = 68;                                  // row stride (floats) of the staged accumulators
@@ -732,23 +736,37 @@ struct ColCtx {
   Group<NV> grp;
 };
 
+// accumulator registers of a colour stage per thread: Np / 2 for each 64-row half
+template <int STAGE>
+__host__ __device__ constexpr int col_acc() { return REL_PLAN.st[STAGE].Np; }
+
+// publish the activation tile and issue both halves of stage STAGE as one committed group; d: half 0's accumulators, then half 1's
 template <int STAGE, int NV>
-__device__ __forceinline__ void col_mma(const ColCtx<NV>& c) {
+__device__ __forceinline__ void col_issue(const ColCtx<NV>& c, float* d) {
   constexpr TcPlan plan = REL_PLAN;
   constexpr int Kp = plan.st[STAGE].Kp, Np = plan.st[STAGE].Np;
   const uint32_t b = c.wbase + (plan.st[STAGE].off - plan.st[GEO_NSTAGE].off);
   wg_publish(c.bar_id);
+  tc::wg_fence();
+  tc::wg_mma<Np, Kp / 16>(d, tc::smem_u32(c.A), 2048u, b, (uint32_t)(Np / 8) * 128u, 0u);
+  tc::wg_mma<Np, Kp / 16>(d + Np / 2, tc::smem_u32(c.A) + 1024u, 2048u, b, (uint32_t)(Np / 8) * 128u, 0u);
+  tc::wg_commit();
+}
+// retire the stage: the fence keeps the accumulators' reads after the wait
+template <int N>
+__device__ __forceinline__ void col_retire(float* d) {
+  tc::wg_wait0();
+  tc::fence_regs<N>(d);
+}
+// stage the retired accumulators (N columns) in D for the row threads
+template <int N, int NV>
+__device__ __forceinline__ void col_stage(const ColCtx<NV>& c, const float* d) {
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
-    float d[Np / 2];
-    tc::wg_fence();
-    tc::wg_mma<Np, Kp / 16>(d, tc::smem_u32(c.A) + 1024u * (uint32_t)half, 2048u, b, (uint32_t)(Np / 8) * 128u, 0u);
-    tc::wg_commit();
-    tc::wg_wait0();
 #pragma unroll
-    for (int m = 0; m < Np / 4; ++m) {
+    for (int m = 0; m < N / 4; ++m) {
       const int r = 64 * half + 16 * c.wq + (c.lane >> 2) + 8 * (m & 1), col = 8 * (m >> 1) + 2 * (c.lane & 3);
-      *reinterpret_cast<float2*>(c.D + r * CDS + col) = make_float2(d[2 * m], d[2 * m + 1]);
+      *reinterpret_cast<float2*>(c.D + r * CDS + col) = make_float2(d[half * N / 2 + 2 * m], d[half * N / 2 + 2 * m + 1]);
     }
   }
   tc::named_sync(c.bar_id, 128);   // accumulators staged, every MMA has read the activation tile
@@ -761,77 +779,116 @@ __device__ __forceinline__ void d_get(const ColCtx<NV>& c, int c0, float* x) {
     x[i] = f.x; x[i + 1] = f.y; x[i + 2] = f.z; x[i + 3] = f.w;
   }
 }
-// staged accumulator columns [0, 32*NCH) -> act(acc + bias) as the next input's words [0, 16*NCH)
-template <int NCH, int ACT, int NV>  // ACT 1 = softplus100, 2 = ELU
-__device__ __forceinline__ void col_epi(const ColCtx<NV>& c, const float* __restrict__ bias) {
+// ELU(acc + bias) of the retired accumulators (N columns) as the next input's words [0, N / 2), written from the fragments: the word
+// of columns 2w, 2w + 1 of a row is the pair the row thread packed from the staged row before
+template <int N, int NV>
+__device__ __forceinline__ void col_epi_elu(const ColCtx<NV>& c, const float* d, const float* __restrict__ bias) {
+  tc::named_sync(c.bar_id, 128);   // every warp's MMAs have read the activation tile
 #pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    float x[32];
-    d_get<32>(c, 32 * ch, x);
-    uint32_t o[16];
+  for (int half = 0; half < 2; ++half) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float x0 = x[2 * i] + bias[ch * 32 + 2 * i], x1 = x[2 * i + 1] + bias[ch * 32 + 2 * i + 1];
-      if (ACT == 1) { x0 = sp_fast(x0); x1 = sp_fast(x1); }
-      else { x0 = elu_fast(x0); x1 = elu_fast(x1); }
-      o[i] = tc::pack_h2(x0, x1);
+    for (int m = 0; m < N / 4; ++m) {
+      const int r = 64 * half + 16 * c.wq + (c.lane >> 2) + 8 * (m & 1), col = 8 * (m >> 1) + 2 * (c.lane & 3);
+      const float x0 = d[half * N / 2 + 2 * m] + bias[col], x1 = d[half * N / 2 + 2 * m + 1] + bias[col + 1];
+      *reinterpret_cast<uint32_t*>(c.A + tc::a_word_off<128>(r, col >> 1)) = tc::pack_h2(elu_fast(x0), elu_fast(x1));
     }
-    a_put<128, 16>(c.A, c.row, 16 * ch, o);
   }
 }
 
-// Colour pass for one tile of the second work list (entries: x = slot of the latent in the scratch buffer, y = sample id).
+// The four bilinear taps of NC4 float4 groups of one view (gather_f32's addresses), loaded now and blended later with gather_f32's
+// expression, so that the loads are in flight while the tile before runs its last stage.
+template <int NC4>
+struct TapLoads {
+  float4 x[4][NC4];
+  float w00, w01, w10, w11;
+  __device__ __forceinline__ void issue(const MapDesc& m, int v, float u, float vv) {
+    const Taps t = make_taps(u, vv, m.W, m.H);
+    const int c4 = m.C >> 2;
+    const float4* base = (const float4*)m.ptr + (size_t)v * m.H * m.W * c4;
+    const int o[4] = {t.o00, t.o01, t.o10, t.o11};
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int i = 0; i < NC4; ++i) x[k][i] = __ldg(base + (size_t)o[k] * c4 + i);
+    w00 = t.w00; w01 = t.w01; w10 = t.w10; w11 = t.w11;
+  }
+  __device__ __forceinline__ void blend(float* out) const {
+#pragma unroll
+    for (int i = 0; i < NC4; ++i) {
+      const float4 a = x[0][i], b = x[1][i], c = x[2][i], d = x[3][i];
+      out[4 * i + 0] = a.x * w00 + b.x * w01 + c.x * w10 + d.x * w11;
+      out[4 * i + 1] = a.y * w00 + b.y * w01 + c.y * w10 + d.y * w11;
+      out[4 * i + 2] = a.z * w00 + b.z * w01 + c.z * w10 + d.z * w11;
+      out[4 * i + 3] = a.w * w00 + b.w * w01 + c.w * w10 + d.w * w11;
+    }
+  }
+};
+
+// A colour tile's inputs that do not depend on the MLPs, per row (sample, view)
+struct ColIn {
+  int slot, id;          // work-list entry: index into the first work list (latent slot), sample id
+  float rd[4];           // [unit(dir - dir_src), dir . dir_src], reference src/model.py:825-832
+  float rgb[3], t8[8];   // img and feat_tex taps, blended
+  uint32_t lat[12];      // compressed latent, fp16 pairs
+};
+
+// Work-list entry of tile sample si (x = index into the first work list, where the latent sits and, + list_base, where the colour
+// goes; y = sample id).  Query mode shades every valid sample: the first list itself is the work list.  Past the end the index is
+// clamped to the last entry (the row computes and writes nothing).
+__device__ __forceinline__ int2 col_entry(const int2* __restrict__ list2, const int* __restrict__ list1, int count, int si) {
+  const int e = min(si, count - 1);
+  return list2 ? list2[e] : make_int2(e, list1[e]);
+}
+// the ray difference and the projection (u, vv) of sample p seen from view v
+template <int NV>
+__device__ __forceinline__ void col_ray(const SceneS<NV>& sc, int v, const float p[3], const float d[3], float rd[4], float& u,
+                                        float& vv) {
+  const Proj q = project_s(sc, v, p);
+  u = q.u; vv = q.v;
+  float r[3] = {p[0] - sc.C[v][0], p[1] - sc.C[v][1], p[2] - sc.C[v][2]};
+  float n = fmaxf(sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2]), 1e-12f);
+  r[0] /= n; r[1] /= n; r[2] /= n;
+  float e[3] = {d[0] - r[0], d[1] - r[1], d[2] - r[2]};
+  float en = fmaxf(sqrtf(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), 1e-6f);
+  rd[0] = e[0] / en; rd[1] = e[1] / en; rd[2] = e[2] / en;
+  rd[3] = r[0] * d[0] + r[1] * d[1] + r[2] * d[2];
+}
+__device__ __forceinline__ void col_lat_issue(const uint4* __restrict__ lat_in, int slot, uint4 w[3]) {
+  w[0] = __ldg(lat_in + 3ll * slot + 0); w[1] = __ldg(lat_in + 3ll * slot + 1); w[2] = __ldg(lat_in + 3ll * slot + 2);
+}
+__device__ __forceinline__ void col_in_finish(const TapLoads<1>& li, const TapLoads<2>& lt, const uint4 w[3], ColIn& in) {
+  float c4[4];
+  li.blend(c4);
+  in.rgb[0] = c4[0]; in.rgb[1] = c4[1]; in.rgb[2] = c4[2];
+  lt.blend(in.t8);
+  const uint32_t* wl = reinterpret_cast<const uint32_t*>(w);
+#pragma unroll
+  for (int i = 0; i < 12; ++i) in.lat[i] = wl[i];
+}
+
+// Colour pass of one tile (reference src/model.py:806-832, 1279-1301) from its prefetched inputs `in`; beside its stages the row
+// threads fetch the inputs of tile sample sn of the next tile into `nx`.  The next tile's inputs are fetched whether or not there is
+// one (col_entry clamps the index), so that no branch separates a wgmma chain from its wait.
 template <int NV>
 __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts& C, const SampleSrc& src,
-                                           const int2* __restrict__ list2, const int* __restrict__ list1, int count, int tile,
-                                           const ColCtx<NV>& cx, const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
-  constexpr int SPW = spw(NV), SPT = spt(NV);
+                                           const int2* __restrict__ list2, const int* __restrict__ list1, int count, int si,
+                                           const ColIn& in, int sn, ColIn& nx, const ColCtx<NV>& cx,
+                                           const uint4* __restrict__ lat_in, int query_mode, const ShadeOut& so) {
+  constexpr int SPW = spw(NV);
   const int lane = cx.lane;
   const int g = lane / NV;
   const int v = lane - NV * g;
-  const int si = tile * SPT + cx.wq * SPW + min(g, SPW - 1);
   const bool writer = (lane < NV * SPW) && (v == 0) && (si < count);
-  // entry: x = index into the first work list (where the latent sits and, + list_base, where the colour goes), y = sample id;
-  // query mode shades every valid sample: the first list itself is the work list
-  const int e = min(si, count - 1);
-  const int2 ent = list2 ? list2[e] : make_int2(e, list1[e]);
-  const int id = ent.y;
-  float p[3], d[3];
-  fetch_sample(src, id, p, d);
-  const Proj q = project_s(sc, v, p);
-  float lat[24];
-  {
-    uint4 w[3];
-    w[0] = __ldg(lat_in + 3ll * ent.x + 0); w[1] = __ldg(lat_in + 3ll * ent.x + 1); w[2] = __ldg(lat_in + 3ll * ent.x + 2);
-    const __half2* hp = reinterpret_cast<const __half2*>(w);
+  float f[35];
+  f[0] = in.rgb[0]; f[1] = in.rgb[1]; f[2] = in.rgb[2];
 #pragma unroll
-    for (int i = 0; i < 12; ++i) { float2 t2 = __half22float2(hp[i]); lat[2 * i] = t2.x; lat[2 * i + 1] = t2.y; }
+  for (int i = 0; i < 8; ++i) f[3 + i] = in.t8[i];
+#pragma unroll
+  for (int i = 0; i < 12; ++i) {
+    const float2 t2 = __half22float2(*reinterpret_cast<const __half2*>(&in.lat[i]));
+    f[11 + 2 * i] = t2.x; f[12 + 2 * i] = t2.y;
   }
-  // ---- colour branch inputs (src/model.py:806-832)
-  float rgb[3], f[35], rd[4];
-  {
-    const Taps ti = make_taps(q.u, q.v, sc.img.W, sc.img.H);
-    float c4[4];
-    gather_f32<1>(sc.img, v, ti, 0, c4);
-    rgb[0] = c4[0]; rgb[1] = c4[1]; rgb[2] = c4[2];
-    f[0] = c4[0]; f[1] = c4[1]; f[2] = c4[2];
-    const Taps tt = make_taps(q.u, q.v, sc.ftex.W, sc.ftex.H);
-    float t8[8];
-    gather_f32<2>(sc.ftex, v, tt, 0, t8);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[3 + i] = t8[i];
-#pragma unroll
-    for (int i = 0; i < 24; ++i) f[11 + i] = lat[i];
-    {  // [unit(dir - dir_src), dir . dir_src], reference src/model.py:825-832
-      float r[3] = {p[0] - sc.C[v][0], p[1] - sc.C[v][1], p[2] - sc.C[v][2]};
-      float n = fmaxf(sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2]), 1e-12f);
-      r[0] /= n; r[1] /= n; r[2] /= n;
-      float e[3] = {d[0] - r[0], d[1] - r[1], d[2] - r[2]};
-      float en = fmaxf(sqrtf(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), 1e-6f);
-      rd[0] = e[0] / en; rd[1] = e[1] / en; rd[2] = e[2] / en;
-      rd[3] = r[0] * d[0] + r[1] * d[1] + r[2] * d[2];
-    }
-  }
+  int2 en;
   {  // ray-direction encoder 4->16->35, ELU, added onto the features (src/model.py:1279-1284): first layer in fp32 on the CUDA
      // cores, second layer (stage 12, bias as K row 16) on the tensor core
     uint32_t a[16];
@@ -839,14 +896,18 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
     for (int o = 0; o < 16; o += 2) {
       float acc0 = C.b_re0[o], acc1 = C.b_re0[o + 1];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { acc0 = fmaf(C.w_re0[o][i], rd[i], acc0); acc1 = fmaf(C.w_re0[o + 1][i], rd[i], acc1); }
+      for (int i = 0; i < 4; ++i) { acc0 = fmaf(C.w_re0[o][i], in.rd[i], acc0); acc1 = fmaf(C.w_re0[o + 1][i], in.rd[i], acc1); }
       a[o / 2] = tc::pack_h2(elu_fast(acc0), elu_fast(acc1));
     }
     a[8] = H2_ONE;   // bias column
 #pragma unroll
     for (int i = 9; i < 16; ++i) a[i] = 0u;
     a_put<128, 16>(cx.A, cx.row, 0, a);
-    col_mma<12>(cx);
+    float d[col_acc<12>()];
+    col_issue<12>(cx, d);
+    en = col_entry(list2, list1, count, sn);
+    col_retire<col_acc<12>()>(d);
+    col_stage<col_acc<12>()>(cx, d);
     float r[36];
     d_get<36>(cx, 0, r);
 #pragma unroll
@@ -854,7 +915,7 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
   }
   float om;  // blending weight (src/model.py:1286-1289), mask == 1
   {
-    float ex = ex2f(C.ani_abs * LOG2E * (rd[3] - 1.0f));
+    float ex = ex2f(C.ani_abs * LOG2E * (in.rd[3] - 1.0f));
     float e = ex - cx.grp.vmin(ex);
     om = e / (cx.grp.sum(e) + 1e-8f);
   }
@@ -878,12 +939,25 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
     }
     a_put<128, 56>(cx.A, cx.row, 0, a);
   }
-  col_mma<6>(cx);
   // ---- BASE0 -> BASE1
-  col_epi<2, 2>(cx, C.b_base0);
-  col_mma<7>(cx);
+  float pn[3], dn[3];
+  uint4 lw[3];
+  {
+    float d[col_acc<6>()];
+    col_issue<6>(cx, d);
+    fetch_sample(src, en.y, pn, dn);
+    col_lat_issue(lat_in, en.x, lw);
+    col_retire<col_acc<6>()>(d);
+    col_epi_elu<col_acc<6>()>(cx, d, C.b_base0);
+  }
+  float un, vn;
   float x[32];
   {
+    float d[col_acc<7>()];
+    col_issue<7>(cx, d);
+    col_ray(sc, v, pn, dn, nx.rd, un, vn);
+    col_retire<col_acc<7>()>(d);
+    col_stage<col_acc<7>()>(cx, d);
     float r[32];
     d_get<32>(cx, 0, r);
     uint32_t o[16];
@@ -893,11 +967,18 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * om, x[2 * i + 1] * om);  // vis_layer1(x * weight)
     a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  col_mma<8>(cx);
   // ---- VIS1A -> VIS1B (src/model.py:1294-1296)
-  col_epi<1, 2>(cx, C.b_vis1a);
-  col_mma<9>(cx);
   {
+    float d[col_acc<8>()];
+    col_issue<8>(cx, d);
+    col_retire<col_acc<8>()>(d);
+    col_epi_elu<col_acc<8>()>(cx, d, C.b_vis1a);
+  }
+  {
+    float d[col_acc<9>()];
+    col_issue<9>(cx, d);
+    col_retire<col_acc<9>()>(d);
+    col_stage<col_acc<9>()>(cx, d);
     float r[36];
     d_get<36>(cx, 0, r);
     float sg = sig_fast(elu_fast(r[32] + C.b_vis1b[32]));
@@ -908,9 +989,12 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i] * sg, x[2 * i + 1] * sg);  // x * sigmoid(vis) * mask
     a_put<128, 16>(cx.A, cx.row, 0, o);
   }
-  col_mma<10>(cx);
   // ---- VIS2A (+ 32->1 sigmoid on CUDA cores) -> OUT0 input [x32 | vis | ray_diff4 | 0-pad] (src/model.py:1297-1300)
   {
+    float d[col_acc<10>()];
+    col_issue<10>(cx, d);
+    col_retire<col_acc<10>()>(d);
+    col_stage<col_acc<10>()>(cx, d);
     float r[32];
     d_get<32>(cx, 0, r);
     float dot = C.b_vis2b;
@@ -920,17 +1004,24 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
     uint32_t o[24];
 #pragma unroll
     for (int i = 0; i < 16; ++i) o[i] = tc::pack_h2(x[2 * i], x[2 * i + 1]);
-    o[16] = tc::pack_h2(vis2, rd[0]);
-    o[17] = tc::pack_h2(rd[1], rd[2]);
-    o[18] = tc::pack_h2(rd[3], 0.0f);
+    o[16] = tc::pack_h2(vis2, in.rd[0]);
+    o[17] = tc::pack_h2(in.rd[1], in.rd[2]);
+    o[18] = tc::pack_h2(in.rd[3], 0.0f);
 #pragma unroll
     for (int i = 19; i < 24; ++i) o[i] = 0u;
     a_put<128, 24>(cx.A, cx.row, 0, o);
   }
-  col_mma<11>(cx);
   // ---- OUT0 -> 16->8->1 on CUDA cores -> softmax over the views -> blended colour (src/model.py:1300-1301)
+  TapLoads<1> li;
+  TapLoads<2> lt;
   float logit;
   {
+    float d[col_acc<11>()];
+    col_issue<11>(cx, d);
+    li.issue(sc.img, v, un, vn);
+    lt.issue(sc.ftex, v, un, vn);
+    col_retire<col_acc<11>()>(d);
+    col_stage<col_acc<11>()>(cx, d);
     float r[16];
     d_get<16>(cx, 0, r);
     float h16[16];
@@ -948,12 +1039,14 @@ __device__ __forceinline__ void color_tile(const SceneS<NV>& sc, const TcConsts&
   {
     float e = ex2f((logit - cx.grp.vmax(logit)) * LOG2E);
     float inv = 1.0f / cx.grp.sum(e);
-    float r0 = cx.grp.sum(e * rgb[0]) * inv, r1 = cx.grp.sum(e * rgb[1]) * inv, r2 = cx.grp.sum(e * rgb[2]) * inv;
+    float r0 = cx.grp.sum(e * in.rgb[0]) * inv, r1 = cx.grp.sum(e * in.rgb[1]) * inv, r2 = cx.grp.sum(e * in.rgb[2]) * inv;
     if (writer) {
-      float* o = query_mode ? so.out5 + 5ll * id + 2 : so.rgb + 3ll * (so.list_base + ent.x);
+      float* o = query_mode ? so.out5 + 5ll * in.id + 2 : so.rgb + 3ll * (so.list_base + in.slot);
       o[0] = r0; o[1] = r1; o[2] = r2;
     }
   }
+  nx.slot = en.x; nx.id = en.y;
+  col_in_finish(li, lt, lw, nx);
 }
 
 // wcol: the blob's tile of stage 6 (the colour stages' tiles follow it)
@@ -966,7 +1059,7 @@ shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcC
   __shared__ uint64_t wbar;
   __shared__ SceneS<NV> scs;
   constexpr TcPlan plan = REL_PLAN;
-  constexpr int SPT = spt(NV);
+  constexpr int SPW = spw(NV), SPT = spt(NV);
   constexpr uint32_t WBYTES = plan.total_bytes - plan.st[GEO_NSTAGE].off;
   constexpr uint32_t WPAD = (WBYTES + 1023u) / 1024u * 1024u;
   const int t = threadIdx.x, wg = t >> 7;
@@ -982,8 +1075,34 @@ shade_color_kernel(const DevScene* __restrict__ scp, const __grid_constant__ TcC
   ColCtx<NV> cx{wsm + WPAD + (size_t)wg * (CA_BYTES + CD_BYTES), nullptr, tc::smem_u32(wsm), 1 + wg, t & 127, (t >> 5) & 3, lane,
                 Group<NV>(lane)};
   cx.D = reinterpret_cast<float*>(cx.A + CA_BYTES);
-  for (int tile = blockIdx.x * CWG + wg; tile < ntiles; tile += gridDim.x * CWG)
-    color_tile(scs, C, src, list2, list1, count, tile, cx, lat_in, query_mode, so);
+  const int g = lane / NV, v = lane - NV * g;
+  const int srow = cx.wq * SPW + min(g, SPW - 1);   // this lane's sample within a tile
+  const int tstride = gridDim.x * CWG;
+  int tile = blockIdx.x * CWG + wg;
+  if (tile >= ntiles) return;
+  ColIn in;
+  {  // the first tile's inputs
+    const int2 e = col_entry(list2, list1, count, tile * SPT + srow);
+    in.slot = e.x; in.id = e.y;
+    float p[3], d[3], u, vv;
+    fetch_sample(src, e.y, p, d);
+    col_ray(scs, v, p, d, in.rd, u, vv);
+    TapLoads<1> li;
+    TapLoads<2> lt;
+    uint4 lw[3];
+    col_lat_issue(lat_in, e.x, lw);
+    li.issue(scs.img, v, u, vv);
+    lt.issue(scs.ftex, v, u, vv);
+    col_in_finish(li, lt, lw, in);
+  }
+  for (;;) {
+    const int next = tile + tstride;
+    ColIn nx;
+    color_tile(scs, C, src, list2, list1, count, tile * SPT + srow, in, next * SPT + srow, nx, cx, lat_in, query_mode, so);
+    if (next >= ntiles) break;
+    tile = next;
+    in = nx;
+  }
 }
 
 }  // namespace

@@ -12,7 +12,10 @@ card's name, power limit and maximum SM clock are read in the same run and print
 The line also sets geo_tail_kernel's time against the two floors its shapes give, at the H100 SXM data sheet's rates (3.35 TB/s
 HBM3, 989 TFLOP/s dense fp16; figures the card is not claimed to reach): the bytes it must move (the 512-byte pooled row of every
 valid sample in, its 8-byte alpha / sdf record and, for samples with density > 0, the 48-byte latent out) and the MMA work it
-executes (per 64-sample tile, engine 0: P0|compress 26 m64n96k16 and P1 14 m64n64k16).
+executes (per 64-sample tile, engine 0: P0|compress 26 m64n96k16 and P1 14 m64n64k16).  shade_color_kernel (colour_list
+reported beside it) is set against the same two floors: the MMA work it executes (128 rows x 15 104 MAC per tile of 40 samples,
+3 views) and the bytes its loads and stores request (per coloured sample: the 8-byte work-list entry, the ray's 32 bytes, the
+48-byte latent, four 16-byte img and four 32-byte feat_tex taps per view, and the 12-byte colour out).
 """
 from __future__ import annotations
 
@@ -33,6 +36,8 @@ GROUPS = ("geo_front_kernel", "geo_tail_kernel", "colour_list", "shade_color_ker
 DATASHEET_BYTES_S = 3.35e12   # H100 SXM, HBM3
 DATASHEET_FLOP_S = 989e12     # H100 SXM, dense fp16 tensor
 TAIL_TILE_FLOP = 2 * 64 * 16 * (26 * 96 + 14 * 64)   # executed MMA work of one 64-sample tile with two-term weights (engine 0)
+# executed MMA work of one colour tile (128 rows): sum of Kp x Np over RE1, BASE0, BASE1, VIS1A, VIS1B, VIS2A, OUT0
+COLOUR_TILE_FLOP = 2 * 128 * (32 * 48 + 112 * 64 + 64 * 32 + 32 * 32 + 32 * 48 + 32 * 32 + 48 * 16)
 
 
 def tail_floors(valid: int, coloured: int, tail_ms: float) -> dict:
@@ -44,6 +49,18 @@ def tail_floors(valid: int, coloured: int, tail_ms: float) -> dict:
             "datasheet_GB_s": DATASHEET_BYTES_S / 1e9, "byte_floor_ms": round(nbytes / DATASHEET_BYTES_S * 1e3, 3),
             "executed_mma_flop": flop, "achieved_TFLOP_s": round(flop / s / 1e12, 1) if s else None,
             "datasheet_TFLOP_s": DATASHEET_FLOP_S / 1e12, "mma_floor_ms": round(flop / DATASHEET_FLOP_S * 1e3, 3)}
+
+
+def colour_floors(coloured: int, n_views: int, list_ms: float, colour_ms: float) -> dict:
+    """shade_color_kernel against the data sheet: the bytes its loads and stores request and the MMA work it executes."""
+    spt = 4 * (32 // n_views)
+    nbytes = coloured * (8 + 32 + 48 + 12 + n_views * 4 * (16 + 32))
+    flop = COLOUR_TILE_FLOP * ((coloured + spt - 1) // spt)
+    s = colour_ms * 1e-3
+    return {"colour_list_ms": round(list_ms, 3), "shade_color_kernel_ms": round(colour_ms, 3), "requested_bytes": nbytes,
+            "achieved_GB_s": round(nbytes / s / 1e9, 1) if s else None, "byte_floor_ms": round(nbytes / DATASHEET_BYTES_S * 1e3, 3),
+            "executed_mma_flop": flop, "achieved_TFLOP_s": round(flop / s / 1e12, 1) if s else None,
+            "mma_floor_ms": round(flop / DATASHEET_FLOP_S * 1e3, 3)}
 
 
 def card():
@@ -137,7 +154,8 @@ def main():
             "ms_per_frame": {k: round(v, 3) for k, v in ms.items()},
             "flush_ms_excluded": round(sum(flush_us.values()) / 1e3 / args.steps, 3),
             "geometry_ms": round(geo, 3), "front_share_of_geometry": round(ms["geo_front_kernel"] / geo, 3) if geo else None,
-            "tail_vs_datasheet": tail_floors(int(st["samples_valid"]), int(st["samples_coloured"]), ms["geo_tail_kernel"])}
+            "tail_vs_datasheet": tail_floors(int(st["samples_valid"]), int(st["samples_coloured"]), ms["geo_tail_kernel"]),
+            "colour_vs_datasheet": colour_floors(int(st["samples_coloured"]), 3, ms["colour_list"], ms["shade_color_kernel"])}
     m.check_health()
     print(json.dumps(line), flush=True)
     if args.out:
