@@ -22,6 +22,36 @@ __device__ __forceinline__ float linspace01(int i, int S) {
 // depth of coarse sample s of a ray: z = near + (far - near) * linspace(0,1,S)[s]  (reference src/model.py:1045-1055)
 __device__ __forceinline__ float coarse_depth(float n_r, float f_r, int s, int S) { return n_r + (f_r - n_r) * linspace01(s, S); }
 
+// Compositing (reference src/model.py:1150-1176), shared by composite_kernel and its backward.  The list entry at sample k of a
+// ray of S samples: its depth (zz: the ray's depths, else the coarse depths between n_r and f_r), the distance to the next
+// sample (1e10 on the ray's last, reference src/model.py:1166) and its alpha 1 - exp(-sigma dist).
+struct ListEntry { float z, dist, alpha; };
+__device__ __forceinline__ ListEntry list_entry(const float* zz, float n_r, float f_r, int k, int S, float sigma) {
+  ListEntry en;
+  float znext;
+  if (zz) { en.z = zz[k]; znext = k + 1 < S ? zz[k + 1] : 0.0f; }
+  else { en.z = coarse_depth(n_r, f_r, k, S); znext = k + 1 < S ? coarse_depth(n_r, f_r, k + 1, S) : 0.0f; }
+  en.dist = k + 1 < S ? znext - en.z : 1e10f;
+  en.alpha = 1.0f - expf(-sigma * en.dist);
+  return en;
+}
+// Compositing weights of a group of 32 list entries (lane l: entry l, alpha a): c_l = a T_l with the transmittance
+// T_l = Tc prod_{j<l} (1 - a_j), an exclusive product scan across the lanes.  Tc is carried on to the next group.
+__device__ __forceinline__ float composite_weight(float a, int lane, float& Tc, float& T) {
+  float p = 1.0f - a;   // inclusive product scan of (1 - a)
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const float t = __shfl_up_sync(0xffffffffu, p, d);
+    if (lane >= d) p *= t;
+  }
+  float ex = __shfl_up_sync(0xffffffffu, p, 1);
+  if (lane == 0) ex = 1.0f;
+  T = Tc * ex;
+  const float c = a * T;
+  Tc *= __shfl_sync(0xffffffffu, p, 31);
+  return c;
+}
+
 __device__ __forceinline__ float sample_depth(const SampleSrc& src, long long id, long long r) {
   if (src.z) return src.z[id];
   return coarse_depth(src.ray_nf[2 * r], src.ray_nf[2 * r + 1], (int)(id - r * src.S), src.S);

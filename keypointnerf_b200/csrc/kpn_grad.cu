@@ -2,9 +2,9 @@
 // with torch autograd's semantics): the gradient of a loss of one pass' per-ray outputs with respect to every hot-path layer,
 // mlp_tex.ani_al and the three gathered feature maps.
 //
-//   composite_backward   one warp per ray, mirroring composite_kernel: dL/d(colour, alpha, depth, sdf) of the ray -> per list
-//                        position d rad, d sdf_raw, d rgb
-//   shade_simt_backward  tiles of GTS valid samples: recomputes shade_simt_kernel's forward with the same dense_tile arithmetic,
+//   composite_backward   one warp per ray, on composite_kernel's list_entry / composite_weight (kpn_device.cuh): dL/d(colour,
+//                        alpha, depth, sdf) of the ray -> per list position d rad, d sdf_raw, d rgb
+//   shade_simt_backward  tiles of GTS valid samples: recomputes shade_simt_kernel's forward by calling its phases (kpn_simt.cuh),
 //                        then backpropagates colour head -> density head -> view pooling -> per-view geometry MLP (each view's
 //                        activations rebuilt in turn); dW / db into the CTA's own slice, feature-map taps scattered with atomics
 //   grad_reduce          the CTA slices summed in CTA order (deterministic)
@@ -41,12 +41,6 @@ composite_backward_kernel(const int* __restrict__ list, const float2* __restrict
     const float* zz = zbuf ? zbuf + (long long)i * S : nullptr;
     const float n_r = zbuf ? 0.0f : ray_nf[2 * i], f_r = zbuf ? 0.0f : ray_nf[2 * i + 1];
     const int start = start_[i], cnt = cnt_[i];
-    auto depth_and_dist = [&](int k, float& zk, float& dist) {
-      float znext;
-      if (zz) { zk = zz[k]; znext = k + 1 < S ? zz[k + 1] : 0.0f; }
-      else { zk = coarse_depth(n_r, f_r, k, S); znext = k + 1 < S ? coarse_depth(n_r, f_r, k + 1, S) : 0.0f; }
-      dist = k + 1 < S ? znext - zk : 1e10f;
-    };
     // ---- sweep 1 (composite_kernel's arithmetic): the ray's sums; a_k and T_k of every entry go to `at`
     float Tc = 1.0f, acc = 0.0f, cd = 0.0f, cs = 0.0f;
     for (int e0 = 0; e0 < cnt; e0 += 32) {
@@ -56,22 +50,12 @@ composite_backward_kernel(const int* __restrict__ list, const float2* __restrict
       if (live) {
         const int k = list[e] - i * S;
         const float2 as = ao[e];
-        float dist;
-        depth_and_dist(k, zk, dist);
-        a = 1.0f - expf(-as.x * dist);
+        const ListEntry en = list_entry(zz, n_r, f_r, k, S, as.x);
+        zk = en.z; a = en.alpha;
         q1 = as.y;
       }
-      float p = 1.0f - a;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const float t = __shfl_up_sync(FULL, p, d);
-        if (lane >= d) p *= t;
-      }
-      float ex = __shfl_up_sync(FULL, p, 1);
-      if (lane == 0) ex = 1.0f;
-      const float T = Tc * ex;
-      const float c = a * T;
-      Tc *= __shfl_sync(FULL, p, 31);
+      float T;
+      const float c = composite_weight(a, lane, Tc, T);
       if (live) { acc += c; cd += c * zk; cs += c * q1; at[e] = make_float2(a, T); }
     }
 #pragma unroll
@@ -92,7 +76,8 @@ composite_backward_kernel(const int* __restrict__ list, const float2* __restrict
       if (live) {
         const int k = list[e] - i * S;
         as = ao[e];
-        depth_and_dist(k, zk, dist);
+        const ListEntry en = list_entry(zz, n_r, f_r, k, S, as.x);   // a_k and T_k as sweep 1 stored them, below
+        zk = en.z; dist = en.dist;
         const float2 aT = at[e];
         a = aT.x; T = aT.y;
         if (as.x > 0.0f) { q2 = rgb[3ll * e]; q3 = rgb[3ll * e + 1]; q4 = rgb[3ll * e + 2]; }
@@ -296,26 +281,7 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
   // the per-view geometry MLP up to layer 2 (layer 3's input) for view v: X0, H1, X2 (|| feat8), H3
   auto geo_front = [&](int v) {
     float *X0 = sm + SM::X0, *H1 = sm + SM::H1, *X2 = sm + SM::X2, *H3 = sm + SM::H3;
-    {
-      const int r = t >> 2, q4 = t & 3;
-      const float* uv = sUV + (v * GTS + r) * 4;
-      float* row = X0 + r * LDA;
-      Taps t64 = make_taps(uv[0], uv[1], sc.f64.W, sc.f64.H);
-      float f[16];
-      gather_f32<4>(sc.f64, v, t64, q4 * 4, f);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) row[encd + q4 * 16 + i] = f[i];
-      float c[3];
-      to_camera(sc, v, sPd + r * 8, c);
-      for (int k = q4; k < K; k += 4) encode_kpt(sc, v, k, c, row);
-      if (q4 < 2) {
-        Taps t8 = make_taps(uv[0], uv[1], sc.f8.W, sc.f8.H);
-        float g[4];
-        gather_f32<1>(sc.f8, v, t8, q4, g);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) X2[r * 136 + 128 + q4 * 4 + i] = g[i];
-      }
-    }
+    geo_input<GTS>(sc, v, K, encd, sUV, sPd, {X0, LDA}, {X2 + 128, 136});
     __syncthreads();
     dense_tile<ACT_SP, 4>(W, L_GEO0, X0, LDA, H1, 128);
     __syncthreads();
@@ -325,71 +291,20 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
     __syncthreads();
   };
 
-  // the colour head of view v (reference src/model.py:1292-1300) from Xv = [mean || var || f_v]: every activation kept
-  auto head_forward = [&](int v) {
-    float *Xv = sm + SM::Xv, *MV = sm + SM::MV, *Fv = sm + SM::F + v * GTS * 36, *Om = sm + SM::Om;
-    float *Hb1 = sm + SM::Hb1, *Hx = sm + SM::Hx, *Hs2 = sm + SM::Hs2, *Ht1 = sm + SM::Ht1, *Hpv = sm + SM::Hpv;
-    float *Hxx = sm + SM::Hxx, *Hs3 = sm + SM::Hs3, *Hu1 = sm + SM::Hu1, *Hv2 = sm + SM::Hv2, *Hoin = sm + SM::Hoin;
-    float *Ho1 = sm + SM::Ho1, *Ho2 = sm + SM::Ho2, *RD = sm + SM::RD;
-    for (int idx = t; idx < GTS * 105; idx += GNT) {
-      int r = idx / 105, c = idx % 105;
-      Xv[r * 108 + c] = c < 70 ? MV[r * 72 + c] : Fv[r * 36 + (c - 70)];
-    }
-    __syncthreads();
-    dense_tile<ACT_ELU, 2>(W, L_BASE0, Xv, 108, Hb1, 64);
-    __syncthreads();
-    dense_tile<ACT_ELU, 1>(W, L_BASE1, Hb1, 64, Hx, 32);
-    __syncthreads();
-    for (int idx = t; idx < GTS * 32; idx += GNT) {
-      int r = idx >> 5, c = idx & 31;
-      Hs2[r * 32 + c] = Hx[r * 32 + c] * Om[v * GTS + r];
-    }
-    __syncthreads();
-    dense_tile<ACT_ELU, 1>(W, L_VIS1A, Hs2, 32, Ht1, 32);
-    __syncthreads();
-    dense_tile<ACT_ELU, 2>(W, L_VIS1B, Ht1, 32, Hpv, 36);
-    __syncthreads();
-    for (int idx = t; idx < GTS * 32; idx += GNT) {
-      int r = idx >> 5, c = idx & 31;
-      float x = Hx[r * 32 + c] + Hpv[r * 36 + c];
-      Hxx[r * 32 + c] = x;
-      Hs3[r * 32 + c] = x * sigmoidf(Hpv[r * 36 + 32]);
-    }
-    __syncthreads();
-    dense_tile<ACT_ELU, 1>(W, L_VIS2A, Hs3, 32, Hu1, 32);
-    __syncthreads();
-    dense_tile<ACT_NONE, 1>(W, L_VIS2B, Hu1, 32, Hv2, 1);
-    __syncthreads();
-    for (int idx = t; idx < GTS * 37; idx += GNT) {
-      int r = idx / 37, c = idx % 37;
-      Hoin[r * 40 + c] = c < 32 ? Hxx[r * 32 + c] : (c == 32 ? sigmoidf(Hv2[r]) : RD[(v * GTS + r) * 4 + (c - 33)]);
-    }
-    __syncthreads();
-    dense_tile<ACT_ELU, 1>(W, L_OUT0, Hoin, 40, Ho1, 16);
-    __syncthreads();
-    dense_tile<ACT_ELU, 1>(W, L_OUT1, Ho1, 16, Ho2, 8);
-    __syncthreads();
-  };
-
+  // the colour head of view v with every activation kept
+  const HeadBufs head = {{sm + SM::Xv, 108}, {sm + SM::Hb1, 64}, {sm + SM::Hx, 32},  {sm + SM::Hs2, 32}, {sm + SM::Ht1, 32},
+                         {sm + SM::Hpv, 36}, {sm + SM::Hxx, 32}, {sm + SM::Hs3, 32}, {sm + SM::Hu1, 32}, {sm + SM::Hv2, 1},
+                         {sm + SM::Hoin, 40}, {sm + SM::Ho1, 16}, {sm + SM::Ho2, 8}};
   // the ray encoder of view v: E1 = elu(RE0 rd) (Hb1, ld 16), E = elu(RE1 E1) (Xv, ld 36)
-  auto ray_encoder = [&](int v) {
-    dense_tile<ACT_ELU, 1>(W, L_RE0, sm + SM::RD + v * GTS * 4, 4, sm + SM::Hb1, 16);
-    __syncthreads();
-    dense_tile<ACT_ELU, 2>(W, L_RE1, sm + SM::Hb1, 16, sm + SM::Xv, 36);
-    __syncthreads();
-  };
+  const Buf E1 = {sm + SM::Hb1, 16}, E = {sm + SM::Xv, 36};
 
   for (int tile = blockIdx.x; tile * GTS < count; tile += gridDim.x) {
     const int base = tile * GTS;
     const int nrows = min(GTS, count - base);
-    // ---- 1. the tile's samples (rows past the end replicate the last one and get zero upstream gradients)
+    // ---- 1-2. the tile's samples, projections and view weights; upstream gradients (zero on rows past the end, which replicate
+    // the last one)
+    load_tile<GTS>(sc, V, src, list, base, nrows, sId, sPd, sUV, sPW);
     if (t < GTS) {
-      int id = list[base + min(t, nrows - 1)];
-      sId[t] = id;
-      float p[3], d[3];
-      fetch_sample<true>(src, id, p, d);
-      float* o = sPd + t * 8;
-      o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = d[0]; o[4] = d[1]; o[5] = d[2];
       float* g = sG + t * 8;
       if (t < nrows) {
         const long long pos = (long long)list_base + base + t;
@@ -400,20 +315,6 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
         g[0] = g[1] = g[2] = g[3] = g[4] = 0.0f;
       }
     }
-    __syncthreads();
-    // ---- 2. projections and view weights
-    for (int idx = t; idx < V * GTS; idx += GNT) {
-      int v = idx / GTS, r = idx % GTS;
-      Proj q = project_view(sc, v, sPd + r * 8);
-      float* o = sUV + idx * 4;
-      o[0] = q.u; o[1] = q.v; o[2] = q.zn; o[3] = boundary_weight(q);
-    }
-    __syncthreads();
-    if (t < GTS) {
-      float sum = 0.0f;
-      for (int v = 0; v < V; ++v) sum += sUV[(v * GTS + t) * 4 + 3];
-      for (int v = 0; v < V; ++v) sPW[v * GTS + t] = sUV[(v * GTS + t) * 4 + 3] / (sum + 1e-6f);
-    }
     // ---- 3. per-view geometry MLP outputs
     for (int v = 0; v < V; ++v) {
       geo_front(v);
@@ -421,28 +322,12 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
       __syncthreads();
     }
     // ---- 4. pooling, latent, density head forward and backward
-    {
-      const int r = t >> 2, q4 = t & 3;
-      for (int c = q4 * 16; c < q4 * 16 + 16; ++c) {
-        float mean = 0.0f;
-        for (int v = 0; v < V; ++v) mean += sPW[v * GTS + r] * sY[(v * GTS + r) * 64 + c];
-        float var = 0.0f;
-        for (int v = 0; v < V; ++v) {
-          float dlt = sY[(v * GTS + r) * 64 + c] - mean;
-          var += sPW[v * GTS + r] * dlt * dlt;
-        }
-        sPool[r * 128 + c] = mean;
-        sPool[r * 128 + 64 + c] = var;
-      }
-    }
+    pool_geometry<GTS>(V, sPW, sY, {sPool, 128});
     __syncthreads();
     {
       float *D1 = sm + SM::D1, *D2 = sm + SM::D2, *gA = sm + SM::gA, *gB = sm + SM::gB;
       dense_tile<ACT_NONE, 1>(W, L_CMP, sPool, 128, sLat, 24);
-      dense_tile<ACT_SP, 2>(W, L_DEN0, sPool, 128, D1, 64);
-      __syncthreads();
-      dense_tile<ACT_SP, 2>(W, L_DEN1, D1, 64, D2, 64);
-      __syncthreads();
+      density_hidden<GTS>(W, {sPool, 128}, {D1, 64}, {D2, 64});
       // d [sdf_raw, rad] = sG[:, 0:2]
       accum_dw(slice, lay, W, L_DEN2, sG, 8, D2, 64);
       dense_bwd_x<2>(wrow(L_DEN2), 2, 64, 0, 64, sG, 8, gA, 64);
@@ -461,76 +346,23 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
     // ---- 5. colour branch forward (reference src/model.py:806-832, 1279-1289)
     float *F = sm + SM::F, *dF = sm + SM::dF, *MV = sm + SM::MV, *dMV = sm + SM::dMV, *RD = sm + SM::RD, *RGB = sm + SM::RGB;
     float *Om = sm + SM::Om, *dOm = sm + SM::dOm, *Logit = sm + SM::Logit, *dLogit = sm + SM::dLogit;
-    for (int idx = t; idx < V * GTS; idx += GNT) {
-      int v = idx / GTS, r = idx % GTS;
-      const float* uv = sUV + idx * 4;
-      float* f = F + idx * 36;
-      Taps ti = make_taps(uv[0], uv[1], sc.img.W, sc.img.H);
-      float c4[4];
-      gather_f32<1>(sc.img, v, ti, 0, c4);
-      RGB[idx * 4 + 0] = c4[0]; RGB[idx * 4 + 1] = c4[1]; RGB[idx * 4 + 2] = c4[2];
-      f[0] = c4[0]; f[1] = c4[1]; f[2] = c4[2];
-      Taps tt = make_taps(uv[0], uv[1], sc.ftex.W, sc.ftex.H);
-      float g[8];
-      gather_f32<2>(sc.ftex, v, tt, 0, g);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) f[3 + i] = g[i];
-      ray_diff(sc, v, sPd + r * 8, sPd + r * 8 + 3, RD + idx * 4);
-      dOm[idx] = 0.0f;
-    }
+    for (int idx = t; idx < V * GTS; idx += GNT) dOm[idx] = 0.0f;
     for (int idx = t; idx < GTS * 72; idx += GNT) dMV[idx] = 0.0f;
+    colour_inputs<GTS>(sc, V, sUV, sPd, sLat, F, RGB, RD);
+    add_ray_encoding<GTS>(W, V, RD, E1, E, F);
+    blend_weights<GTS>(W, V, RD, Om);
     __syncthreads();
-    for (int idx = t; idx < V * GTS * 24; idx += GNT) {
-      int c = idx % 24, vr = idx / 24;
-      F[vr * 36 + 11 + c] = sLat[(vr % GTS) * 24 + c];
-    }
-    for (int v = 0; v < V; ++v) {
-      __syncthreads();
-      ray_encoder(v);
-      for (int idx = t; idx < GTS * 35; idx += GNT) {
-        int r = idx / 35, c = idx % 35;
-        F[(v * GTS + r) * 36 + c] += sm[SM::Xv + r * 36 + c];
-      }
-    }
-    if (t < GTS) {
-      float ex[MAXV], mn = 3.0e38f;
-      for (int v = 0; v < V; ++v) {
-        ex[v] = expf(W.ani_al_abs * (RD[(v * GTS + t) * 4 + 3] - 1.0f));
-        mn = fminf(mn, ex[v]);
-      }
-      float sum = 0.0f;
-      for (int v = 0; v < V; ++v) { ex[v] -= mn; sum += ex[v]; }
-      for (int v = 0; v < V; ++v) Om[v * GTS + t] = ex[v] / (sum + 1e-8f);
-    }
-    __syncthreads();
-    for (int idx = t; idx < GTS * 35; idx += GNT) {
-      int r = idx / 35, c = idx % 35;
-      float mean = 0.0f;
-      for (int v = 0; v < V; ++v) mean += F[(v * GTS + r) * 36 + c] * Om[v * GTS + r];
-      float var = 0.0f;
-      for (int v = 0; v < V; ++v) {
-        float dlt = F[(v * GTS + r) * 36 + c] - mean;
-        var += Om[v * GTS + r] * dlt * dlt;
-      }
-      MV[r * 72 + c] = mean;
-      MV[r * 72 + 35 + c] = var;
-    }
+    pool_colour<GTS>(V, F, Om, MV);
     __syncthreads();
     for (int v = 0; v < V; ++v) {
-      head_forward(v);
+      colour_head<GTS>(W, v, MV, F, Om, RD, head);
       dense_tile<ACT_NONE, 1>(W, L_OUT2, sm + SM::Ho2, 8, Logit + v * GTS, 1);
       __syncthreads();
     }
     // ---- 6. softmax blend backward: d logit_v = sm_v (rgb_v - rgb) . d rgb
     if (t < GTS) {
-      float m = -3.0e38f;
-      for (int v = 0; v < V; ++v) m = fmaxf(m, Logit[v * GTS + t]);
-      float den = 0.0f, rgb[3] = {0.f, 0.f, 0.f}, e[MAXV];
-      for (int v = 0; v < V; ++v) {
-        e[v] = expf(Logit[v * GTS + t] - m);
-        den += e[v];
-        for (int c = 0; c < 3; ++c) rgb[c] += e[v] * RGB[(v * GTS + t) * 4 + c];
-      }
+      float e[MAXV], rgb[3];
+      const float den = blend_colours<GTS>(V, Logit, RGB, t, e, rgb);
       const float* g = sG + t * 8 + 2;
       for (int v = 0; v < V; ++v) {
         float s = 0.0f;
@@ -541,7 +373,7 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
     __syncthreads();
     // ---- 7. per-view colour head backward, activations rebuilt view by view
     for (int v = 0; v < V; ++v) {
-      head_forward(v);
+      colour_head<GTS>(W, v, MV, F, Om, RD, head);
       float *Xv = sm + SM::Xv, *Hb1 = sm + SM::Hb1, *Hx = sm + SM::Hx, *Hs2 = sm + SM::Hs2, *Ht1 = sm + SM::Ht1;
       float *Hpv = sm + SM::Hpv, *Hxx = sm + SM::Hxx, *Hs3 = sm + SM::Hs3, *Hu1 = sm + SM::Hu1, *Hoin = sm + SM::Hoin;
       float *Ho1 = sm + SM::Ho1, *Ho2 = sm + SM::Ho2, *GA2 = sm + SM::GA2, *GB2 = sm + SM::GB2, *GC = sm + SM::GC;
@@ -671,12 +503,12 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
     }
     for (int v = 0; v < V; ++v) {
       __syncthreads();
-      ray_encoder(v);
-      float *E1 = sm + SM::Hb1, *E = sm + SM::Xv, *GA2 = sm + SM::GA2, *GB2 = sm + SM::GB2;
+      ray_encoder<GTS>(W, v, RD, E1, E);
+      float *GA2 = sm + SM::GA2, *GB2 = sm + SM::GB2;
       float* dFv = dF + v * GTS * 36;
       for (int idx = t; idx < GTS * 35; idx += GNT) {
         int r = idx / 35, c = idx % 35;
-        GA2[r * 108 + c] = dFv[r * 36 + c] * delu(E[r * 36 + c]);
+        GA2[r * 108 + c] = dFv[r * 36 + c] * delu(E.p[r * 36 + c]);
       }
       for (int idx = t; idx < nrows * 2; idx += GNT) {   // d feat_tex of view v (channels 3..10 of f)
         const int r = idx >> 1, c4 = idx & 1;
@@ -684,10 +516,10 @@ shade_simt_backward_kernel(const DevScene* __restrict__ scp, const DevWeightsF32
         scatter4(gr.d_ftex, sc.ftex, 8, v, sUV[(v * GTS + r) * 4], sUV[(v * GTS + r) * 4 + 1], c4, make_float4(g[0], g[1], g[2], g[3]));
       }
       __syncthreads();
-      accum_dw(slice, lay, W, L_RE1, GA2, 108, E1, 16);
+      accum_dw(slice, lay, W, L_RE1, GA2, 108, E1.p, 16);
       dense_bwd_x<1>(wrow(L_RE1), 35, 16, 0, 16, GA2, 108, GB2, 108);
       __syncthreads();
-      act_bwd<ACT_ELU>(GB2, 108, E1, 16, 16);
+      act_bwd<ACT_ELU>(GB2, 108, E1.p, 16, 16);
       __syncthreads();
       accum_dw(slice, lay, W, L_RE0, GB2, 108, RD + v * GTS * 4, 4);
     }

@@ -502,51 +502,11 @@ shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restr
   for (int tile = blockIdx.x; tile * TS < count; tile += gridDim.x) {
     const int base = tile * TS;
     const int nrows = min(TS, count - base);
-    // ---- 1. fetch the tile's samples (rows past the end replicate the last one)
-    if (t < TS) {
-      int id = list[base + min(t, nrows - 1)];
-      s.Id[t] = id;
-      float p[3], d[3];
-      fetch_sample<true>(src, id, p, d);
-      float* o = s.P + t * 8;
-      o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = d[0]; o[4] = d[1]; o[5] = d[2];
-    }
-    __syncthreads();
-    // ---- 2. projections and view weights (reference src/model.py:713-723,750-759; mask == 1 here)
-    for (int idx = t; idx < V * TS; idx += NT) {
-      int v = idx / TS, r = idx % TS;
-      Proj q = project_view(sc, v, s.P + r * 8);
-      float* o = s.UV + idx * 4;
-      o[0] = q.u; o[1] = q.v; o[2] = q.zn; o[3] = boundary_weight(q);
-    }
-    __syncthreads();
-    if (t < TS) {
-      float sum = 0.0f;
-      for (int v = 0; v < V; ++v) sum += s.UV[(v * TS + t) * 4 + 3];
-      for (int v = 0; v < V; ++v) s.PW[v * TS + t] = s.UV[(v * TS + t) * 4 + 3] / (sum + 1e-6f);
-    }
-    // ---- 3. per-view geometry MLP (reference src/utils.py:691-720)
+    // ---- 1. fetch the tile's samples, projections and view weights
+    load_tile<TS>(sc, V, src, list, base, nrows, s.Id, s.P, s.UV, s.PW);
+    // ---- 2. per-view geometry MLP; layer 0's input is still live in A after layer 1, so the feat8 taps wait in F8
     for (int v = 0; v < V; ++v) {
-      {
-        const int r = t >> 2, q4 = t & 3;
-        const float* uv = s.UV + (v * TS + r) * 4;
-        float* row = s.A + r * LDA;
-        Taps t64 = make_taps(uv[0], uv[1], sc.f64.W, sc.f64.H);
-        float f[16];
-        gather_f32<4>(sc.f64, v, t64, q4 * 4, f);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) row[encd + q4 * 16 + i] = f[i];
-        float c[3];
-        to_camera(sc, v, s.P + r * 8, c);
-        for (int k = q4; k < K; k += 4) encode_kpt(sc, v, k, c, row);
-        if (q4 < 2) {
-          Taps t8 = make_taps(uv[0], uv[1], sc.f8.W, sc.f8.H);
-          float g[4];
-          gather_f32<1>(sc.f8, v, t8, q4, g);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) s.F8[r * 8 + q4 * 4 + i] = g[i];
-        }
-      }
+      geo_input<TS>(sc, v, K, encd, s.UV, s.P, {s.A, LDA}, {s.F8, 8});
       __syncthreads();
       dense_tile<ACT_SP, 4>(W, L_GEO0, s.A, LDA, s.B, LDB);
       __syncthreads();
@@ -558,27 +518,11 @@ shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restr
       dense_tile<ACT_NONE, 2>(W, L_GEO3, s.B, LDB, s.XV + v * TS * 64, 64);
       __syncthreads();
     }
-    // ---- 4. weighted mean || variance over views (reference src/utils.py:722-748), density head
-    {
-      const int r = t >> 2, q4 = t & 3;
-      for (int c = q4 * 16; c < q4 * 16 + 16; ++c) {
-        float mean = 0.0f;
-        for (int v = 0; v < V; ++v) mean += s.PW[v * TS + r] * s.XV[(v * TS + r) * 64 + c];
-        float var = 0.0f;
-        for (int v = 0; v < V; ++v) {
-          float dlt = s.XV[(v * TS + r) * 64 + c] - mean;
-          var += s.PW[v * TS + r] * dlt * dlt;
-        }
-        s.A[r * LDA + c] = mean;
-        s.A[r * LDA + 64 + c] = var;
-      }
-    }
+    // ---- 3. pooling over views, density head
+    pool_geometry<TS>(V, s.PW, s.XV, {s.A, LDA});
     __syncthreads();
     if (query_mode != 2) dense_tile<ACT_NONE, 1>(W, L_CMP, s.A, LDA, s.Lat, 24);   // ibr_compress_gfeat (src/model.py:819)
-    dense_tile<ACT_SP, 2>(W, L_DEN0, s.A, LDA, s.B, LDB);
-    __syncthreads();
-    dense_tile<ACT_SP, 2>(W, L_DEN1, s.B, LDB, s.A, LDA);
-    __syncthreads();
+    density_hidden<TS>(W, {s.A, LDA}, {s.B, LDB}, {s.A, LDA});
     dense_tile<ACT_NONE, 1>(W, L_DEN2, s.A, LDA, s.Geo, 2);
     if (query_mode == 2) {   // geometry only: [sdf_raw, rad], no colour stages
       __syncthreads();
@@ -586,119 +530,26 @@ shade_simt_kernel(const DevScene* __restrict__ scp, const DevWeightsF32* __restr
       __syncthreads();
       continue;
     }
-    // ---- 5. colour branch inputs (reference src/model.py:806-832)
-    for (int idx = t; idx < V * TS; idx += NT) {
-      int v = idx / TS, r = idx % TS;
-      const float* uv = s.UV + idx * 4;
-      float* f = s.F + idx * 36;
-      Taps ti = make_taps(uv[0], uv[1], sc.img.W, sc.img.H);
-      float c4[4];
-      gather_f32<1>(sc.img, v, ti, 0, c4);
-      s.RGB[idx * 4 + 0] = c4[0]; s.RGB[idx * 4 + 1] = c4[1]; s.RGB[idx * 4 + 2] = c4[2];
-      f[0] = c4[0]; f[1] = c4[1]; f[2] = c4[2];
-      Taps tt = make_taps(uv[0], uv[1], sc.ftex.W, sc.ftex.H);
-      float g[8];
-      gather_f32<2>(sc.ftex, v, tt, 0, g);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) f[3 + i] = g[i];
-      ray_diff(sc, v, s.P + r * 8, s.P + r * 8 + 3, s.RD + idx * 4);
-    }
+    // ---- 4. colour branch inputs, ray encoding, blending weights, pooling over views
+    colour_inputs<TS>(sc, V, s.UV, s.P, s.Lat, s.F, s.RGB, s.RD);
+    add_ray_encoding<TS>(W, V, s.RD, {s.B, LDB}, {s.A, LDA}, s.F);
+    blend_weights<TS>(W, V, s.RD, s.Om);
     __syncthreads();
-    for (int idx = t; idx < V * TS * 24; idx += NT) {
-      int c = idx % 24, vr = idx / 24;
-      s.F[vr * 36 + 11 + c] = s.Lat[(vr % TS) * 24 + c];
-    }
-    // ray-direction encoder 4->16->35 (ELU) added onto the features (src/model.py:1279-1284)
+    pool_colour<TS>(V, s.F, s.Om, s.MV);
+    __syncthreads();
+    // ---- 5. per-view IBR head
     for (int v = 0; v < V; ++v) {
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_RE0, s.RD + v * TS * 4, 4, s.B, LDB);
-      __syncthreads();
-      dense_tile<ACT_ELU, 2>(W, L_RE1, s.B, LDB, s.A, LDA);
-      __syncthreads();
-      for (int idx = t; idx < TS * 35; idx += NT) {
-        int r = idx / 35, c = idx % 35;
-        s.F[(v * TS + r) * 36 + c] += s.A[r * LDA + c];
-      }
-    }
-    // blending weights (src/model.py:1286-1289), mask == 1
-    if (t < TS) {
-      float ex[MAXV], mn = 3.0e38f;
-      for (int v = 0; v < V; ++v) {
-        ex[v] = expf(W.ani_al_abs * (s.RD[(v * TS + t) * 4 + 3] - 1.0f));
-        mn = fminf(mn, ex[v]);
-      }
-      float sum = 0.0f;
-      for (int v = 0; v < V; ++v) { ex[v] -= mn; sum += ex[v]; }
-      for (int v = 0; v < V; ++v) s.Om[v * TS + t] = ex[v] / (sum + 1e-8f);
-    }
-    __syncthreads();
-    for (int idx = t; idx < TS * 35; idx += NT) {
-      int r = idx / 35, c = idx % 35;
-      float mean = 0.0f;
-      for (int v = 0; v < V; ++v) mean += s.F[(v * TS + r) * 36 + c] * s.Om[v * TS + r];
-      float var = 0.0f;
-      for (int v = 0; v < V; ++v) {
-        float dlt = s.F[(v * TS + r) * 36 + c] - mean;
-        var += s.Om[v * TS + r] * dlt * dlt;
-      }
-      s.MV[r * 72 + c] = mean;
-      s.MV[r * 72 + 35 + c] = var;
-    }
-    __syncthreads();
-    // ---- 6. per-view IBR head (src/model.py:1292-1300)
-    for (int v = 0; v < V; ++v) {
-      for (int idx = t; idx < TS * 105; idx += NT) {
-        int r = idx / 105, c = idx % 105;
-        s.A[r * LDA + c] = c < 70 ? s.MV[r * 72 + c] : s.F[(v * TS + r) * 36 + (c - 70)];
-      }
-      __syncthreads();
-      dense_tile<ACT_ELU, 2>(W, L_BASE0, s.A, LDA, s.B, LDB);
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_BASE1, s.B, LDB, S1, 64);
-      __syncthreads();
-      for (int idx = t; idx < TS * 32; idx += NT) {
-        int r = idx >> 5, c = idx & 31;
-        S2[r * 64 + c] = S1[r * 64 + c] * s.Om[v * TS + r];
-      }
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_VIS1A, S2, 64, S3, 64);
-      __syncthreads();
-      dense_tile<ACT_ELU, 2>(W, L_VIS1B, S3, 64, S2, 64);
-      __syncthreads();
-      for (int idx = t; idx < TS * 32; idx += NT) {
-        int r = idx >> 5, c = idx & 31;
-        float x = S1[r * 64 + c] + S2[r * 64 + c];
-        S1[r * 64 + c] = x;
-        S3[r * 64 + c] = x * sigmoidf(S2[r * 64 + 32]);
-      }
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_VIS2A, S3, 64, S2, 64);
-      __syncthreads();
-      dense_tile<ACT_NONE, 1>(W, L_VIS2B, S2, 64, s.Vis, 1);
-      __syncthreads();
-      for (int idx = t; idx < TS * 37; idx += NT) {
-        int r = idx / 37, c = idx % 37;
-        float val = c < 32 ? S1[r * 64 + c] : (c == 32 ? sigmoidf(s.Vis[r]) : s.RD[(v * TS + r) * 4 + (c - 33)]);
-        S3[r * 64 + c] = val;
-      }
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_OUT0, S3, 64, S2, 64);
-      __syncthreads();
-      dense_tile<ACT_ELU, 1>(W, L_OUT1, S2, 64, S3, 64);
-      __syncthreads();
+      // the activations in place in S1-S3 (see colour_head)
+      colour_head<TS>(W, v, s.MV, s.F, s.Om, s.RD,
+                      {{s.A, LDA}, {s.B, LDB}, {S1, 64}, {S2, 64}, {S3, 64}, {S2, 64}, {S1, 64}, {S3, 64}, {S2, 64}, {s.Vis, 1},
+                       {S3, 64}, {S2, 64}, {S3, 64}});
       dense_tile<ACT_NONE, 1>(W, L_OUT2, S3, 64, s.Logit + v * TS, 1);
       __syncthreads();
     }
-    // ---- 7. softmax blend of the source colours and output (src/model.py:1300-1301, 978-997)
+    // ---- 6. softmax blend of the source colours and output (src/model.py:1300-1301, 978-997)
     if (t < nrows) {
-      float m = -3.0e38f;
-      for (int v = 0; v < V; ++v) m = fmaxf(m, s.Logit[v * TS + t]);
-      float den = 0.0f, rgb[3] = {0.f, 0.f, 0.f};
-      for (int v = 0; v < V; ++v) {
-        float e = expf(s.Logit[v * TS + t] - m);
-        den += e;
-        for (int c = 0; c < 3; ++c) rgb[c] += e * s.RGB[(v * TS + t) * 4 + c];
-      }
+      float e[MAXV], rgb[3];
+      const float den = blend_colours<TS>(V, s.Logit, s.RGB, t, e, rgb);
       float g0 = s.Geo[t * 2], rad = s.Geo[t * 2 + 1];
       if (query_mode) {
         float* o = so.out5 + 5ll * s.Id[t];
@@ -747,24 +598,13 @@ composite_kernel(const int* __restrict__ list, const float2* __restrict__ ao, co
         if (live) {
           const int k = list[e] - i * S;
           const float2 as = ao[e];
-          float znext;
-          if (zz) { zk = zz[k]; znext = k + 1 < S ? zz[k + 1] : 0.0f; }
-          else { zk = coarse_depth(n_r, f_r, k, S); znext = k + 1 < S ? coarse_depth(n_r, f_r, k + 1, S) : 0.0f; }
-          const float dist = k + 1 < S ? znext - zk : 1e10f;
-          a = 1.0f - expf(-as.x * dist);
+          const ListEntry en = list_entry(zz, n_r, f_r, k, S, as.x);
+          zk = en.z; a = en.alpha;
           q1 = as.y;
           if (as.x > 0.0f) { q2 = rgb[3ll * e]; q3 = rgb[3ll * e + 1]; q4 = rgb[3ll * e + 2]; }   // colour exists iff alpha > 0
         }
-        float p = 1.0f - a;   // inclusive product scan of (1 - a)
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const float t = __shfl_up_sync(0xffffffffu, p, d);
-          if (lane >= d) p *= t;
-        }
-        float ex = __shfl_up_sync(0xffffffffu, p, 1);
-        if (lane == 0) ex = 1.0f;
-        const float c = a * (Tc * ex);
-        Tc *= __shfl_sync(0xffffffffu, p, 31);
+        float T;
+        const float c = composite_weight(a, lane, Tc, T);
         if (live) {
           acc += c; cr += c * q2; cg += c * q3; cb += c * q4; cd += c * zk; cs += c * q1;
           if (cw) cw[e] = c;
